@@ -17,6 +17,7 @@ from .envs import env_ids, make  # noqa: F401
 from .physical_systems import PhysicalSystem  # noqa: F401
 from .reference_generators import ReferenceGenerator  # noqa: F401
 from .reward_functions import RewardFunction, WeightedSumOfErrors  # noqa: F401
+from .snapshot import EnvSnapshot  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -145,7 +145,8 @@ SYMBOLS = [
     "gemb200_destroy", "gemb200_reset", "gemb200_step", "gemb200_step_host", "gemb200_reset_host", "gemb200_rollout", "gemb200_rollout_record",
     "gemb200_get_ode_state", "gemb200_set_ode_state", "gemb200_get_reference", "gemb200_set_reference",
     "gemb200_reseed", "gemb200_set_device_clock", "gemb200_get_clock", "gemb200_set_env_params", "gemb200_peer_buffer_alloc", "gemb200_peer_buffer_open", "gemb200_peer_buffer_close",
-    "gemb200_peer_buffer_free", "gemb200_bind_peers", "gemb200_peer_signal", "gemb200_peer_wait", "gemb200_checkpoint_size", "gemb200_checkpoint_save", "gemb200_checkpoint_load", "gemb200_launch_count",
+    "gemb200_peer_buffer_free", "gemb200_bind_peers", "gemb200_peer_signal", "gemb200_peer_wait", "gemb200_checkpoint_size", "gemb200_checkpoint_save", "gemb200_checkpoint_load", "gemb200_query_env_record",
+    "gemb200_pack_envs", "gemb200_unpack_envs", "gemb200_launch_count",
     "gemb200_kernel_time_begin", "gemb200_kernel_time_end",
 ]
 
@@ -207,6 +208,9 @@ def load_library():
     lib.gemb200_checkpoint_size.restype = C.c_int64
     lib.gemb200_checkpoint_save.argtypes = [vp, vp]
     lib.gemb200_checkpoint_load.argtypes = [vp, vp]
+    lib.gemb200_query_env_record.argtypes = [cfgp, i32p, C.POINTER(C.c_uint64)]
+    lib.gemb200_pack_envs.argtypes = [vp, vp, C.c_int32, vp, vp]
+    lib.gemb200_unpack_envs.argtypes = [vp, vp, C.c_int32, C.c_uint64, vp, vp, C.c_int32, vp]
     lib.gemb200_launch_count.argtypes = [vp]
     lib.gemb200_launch_count.restype = C.c_int64
     lib.gemb200_kernel_time_begin.argtypes = [vp, vp]

@@ -323,6 +323,35 @@ class ElectricMotorEnvironment(_EnvBase):
             lp[:, self._LP_SLOT[name]] = np.broadcast_to(np.asarray(vals, dtype=np.float64), (sim.n,))
         sim.set_env_params(mp, lp)
 
+    def snapshot_envs(self, idx=None):
+        """Branching support, the batched counterpart of `copy.deepcopy(env)`: the complete persistent state of envs `idx` (None: all;
+        list, numpy array or tensor) as an `EnvSnapshot` of packed device rows, taken without a host synchronisation.  Host-side
+        indices are range-checked (IndexError); a device index tensor is taken as given.  Batched mode only."""
+        if self._scalar:
+            raise TypeError("snapshot_envs() needs a batched environment (num_envs=...)")
+        from .snapshot import check_host_index
+
+        sim = self._ensure_sim()
+        return sim.snapshot(check_host_index(idx, sim.n, "idx"))
+
+    def restore_envs(self, snapshot, idx=None, rows=None):
+        """Env idx[j] (None: env j) takes the state of snapshot row rows[j] (None: row j): physically the source env, continuing bit for
+        bit except for the random numbers, which are the restored env's own from then on (its Wiener increments, periodic-generator
+        parameters, switching choices, noise and later random resets).  `rows` fans one snapshot out to many envs without copying it.
+        The snapshot may come from another env of the same kind and record layout (other num_envs or seed); another layout raises
+        ValueError, host-side indices out of range IndexError.  Returns nothing: the observation rows of the restored envs are the
+        caller's to keep (the next step's outputs are computed from the restored state).  Batched mode only."""
+        if self._scalar:
+            raise TypeError("restore_envs() needs a batched environment (num_envs=...)")
+        from .snapshot import check_host_index, check_layout
+
+        sim = self._ensure_sim()
+        words, lid = sim.record_layout()
+        check_layout(snapshot, words, lid)
+        idx = check_host_index(idx, sim.n, "idx")
+        rows = check_host_index(rows, len(snapshot), "rows")
+        sim.restore(snapshot, idx, rows)
+
     def set_reference(self, values):
         """Push reference values [N, n_ref] for ExternalReferenceGenerator slots (used by the next step's reward)."""
         self._ensure_sim().set_reference(values)

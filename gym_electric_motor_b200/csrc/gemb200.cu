@@ -223,6 +223,63 @@ static int validate(const gemb200_config* c) {
   return GEMB200_OK;
 }
 
+// which optional per-env arrays a configuration has (gemb200_create allocates them, sections() lists them)
+static int fifo_dim_of(const gemb200_config* c, const Dims& d) {
+  if (c->dead_time_steps <= 0) return 0;
+  // queue width: caller-side actions when the dead time wraps the dq transformation (or there is none), else abc(+e)
+  const int inner = c->finite ? d.n_act : (d.fam == kDFIM ? 6 : (d.fam == kEESM ? 4 : (d.fam >= kSYNC ? 3 : d.n_act)));
+  return (c->action_dq && !c->dead_time_outer) ? inner : d.n_act;
+}
+static bool has_sw_state(const gemb200_config* c) {  // finite switching states: two-segment steps (interlocking time) or an RC supply
+  return c->finite && (c->interlocking_time > 0 || c->interlocking_time1 > 0 || c->supply_kind == GEMB200_SUPPLY_RC);
+}
+static bool any_switched_slot(const gemb200_config* c) {
+  for (int r = 0; r < c->n_ref; ++r) if (c->ref_sw_count[r] > 1) return true;
+  return false;
+}
+constexpr int kMaxSections = 16;
+// The persistent per-env arrays of a configuration, in checkpoint order.  One table serves the checkpoint blob (ptr, bytes), the reseed
+// and the packed env records of gemb200_pack_envs / gemb200_unpack_envs (element size, elements per env, placement, clock-relative
+// fields), so an array cannot be in one and missing from the other.  h == nullptr: shapes only (ptr = nullptr).
+// checkpoint blob: [header][hot records][cold records][eps][sw][dead-time queue]...  The header pins the blob to the configuration that
+// wrote it: a blob of equal size from another motor / seed / tau / generator set is refused instead of being reinterpreted.
+enum SecPlace { kPlanar = 0, kRecord = 1 };  // planar: element e of env i at [e * n + i]; record: 16-byte chunked record (word_offset)
+enum SecClock {
+  kClkNone = 0,
+  kClkCold = 1,  // cold record: sub-episode ends, and the start step of a slot whose current generator is periodic
+  kClkSwst = 2,  // switched generators [n_ref][2]: the super-episode end (odd elements)
+  kClkRing = 3   // dead-time ring [dead_time_steps][fifo_dim], stored oldest entry first in a row
+};
+struct Section { void* ptr; size_t bytes; int esz, per_env, place, clk; };  // esz: bytes per element
+static int config_sections(const gemb200_config* c, const gemb200_handle* h, Section* s) {
+  Dims d;
+  derive_dims(c, &d);
+  const size_t n = (size_t)c->n_envs;
+  const int rsz = c->dtype == GEMB200_F32 ? 4 : 8;
+  int k = 0;
+  auto add = [&](void* p, int esz, int per_env, int place, int clk) { s[k++] = {p, n * (size_t)per_env * esz, esz, per_env, place, clk}; };
+  add(h ? h->d_st : nullptr, rsz, hot_words(d.nx, c->n_ref), kRecord, kClkNone);
+  add(h ? h->d_stc : nullptr, rsz, cold_words(d.nx, c->n_ref), kRecord, kClkCold);
+  if (d.has_eps) add(h ? h->d_eps : nullptr, 8, 1, kPlanar, kClkNone);
+  if (has_sw_state(c)) add(h ? h->d_sw : nullptr, 2, 1, kPlanar, kClkNone);
+  if (c->dead_time_steps > 0) add(h ? h->d_fifo : nullptr, rsz, c->dead_time_steps * fifo_dim_of(c, d), kPlanar, kClkRing);
+  if (d.has_observer) add(h ? h->d_obsv : nullptr, rsz, 4, kPlanar, kClkNone);
+  if (c->supply_kind == GEMB200_SUPPLY_RC) add(h ? h->d_sup : nullptr, rsz, 2, kPlanar, kClkNone);
+  if (c->supply_kind == GEMB200_SUPPLY_AC1) add(h ? h->d_supph : nullptr, 8, 1, kPlanar, kClkNone);
+  if (any_switched_slot(c)) add(h ? h->d_swst : nullptr, 4, 2 * c->n_ref, kPlanar, kClkSwst);
+  if (c->load_kind == GEMB200_LOAD_EXT_SPEED) add(h ? h->d_kenv : nullptr, 4, 1, kPlanar, kClkNone);
+  if (c->init_im_valid) add(h ? h->d_imprev : nullptr, rsz, 2, kPlanar, kClkNone);
+  return k;  // (the per-env parameter table is configuration, not state: re-apply gemb200_set_env_params after a load)
+}
+static int sections(gemb200_handle* h, Section* s) { return config_sections(&h->cfg, h, s); }
+static bool sections_allocated(gemb200_handle* h) {
+  Section s[kMaxSections];
+  const int k = sections(h, s);
+  for (int q = 0; q < k; ++q) if (!s[q].ptr) return false;
+  return true;
+}
+static int row_words(const Section& s) { return s.per_env * (s.esz == 8 ? 2 : 1); }
+
 // ----------------------------------------------------------------------------------------------------------------
 // model constants (double) -> StepParams<real>
 // ----------------------------------------------------------------------------------------------------------------
@@ -815,13 +872,11 @@ int gemb200_create(const gemb200_config* cfg, gemb200_handle** out) {
   ALLOC(h->d_st, n * (h->NH > 0 ? h->NH : 1) * h->rsz);
   ALLOC(h->d_stc, n * h->NC * h->rsz);
   if (cfg->dead_time_steps > 0) {
-    // queue width: caller-side actions when the dead time wraps the dq transformation (or there is none), else abc(+e)
-    const int inner = cfg->finite ? d.n_act : (d.fam == kDFIM ? 6 : (d.fam == kEESM ? 4 : (d.fam >= kSYNC ? 3 : d.n_act)));
-    h->fifo_dim = (cfg->action_dq && !cfg->dead_time_outer) ? inner : d.n_act;
+    h->fifo_dim = fifo_dim_of(cfg, d);
     ALLOC(h->d_fifo, n * cfg->dead_time_steps * h->fifo_dim * h->rsz);
   }
   if (d.has_eps) ALLOC(h->d_eps, n * sizeof(double));
-  if (h->two_segment || (cfg->finite && cfg->supply_kind == GEMB200_SUPPLY_RC)) ALLOC(h->d_sw, n * sizeof(uint16_t));
+  if (has_sw_state(cfg)) ALLOC(h->d_sw, n * sizeof(uint16_t));
   if (cfg->supply_kind == GEMB200_SUPPLY_RC) ALLOC(h->d_sup, n * 2 * h->rsz);
   if (cfg->supply_kind == GEMB200_SUPPLY_AC1) ALLOC(h->d_supph, n * sizeof(double));
   if (cfg->load_kind == GEMB200_LOAD_EXT_SPEED) {
@@ -845,6 +900,7 @@ int gemb200_create(const gemb200_config* cfg, gemb200_handle** out) {
   if (d.has_observer) ALLOC(h->d_obsv, n * 4 * h->rsz);
   if (cfg->init_im_valid) ALLOC(h->d_imprev, n * 2 * h->rsz);
 #undef ALLOC
+  if (!sections_allocated(h)) { gemb200_destroy(h); return fail(GEMB200_E_INVALID, "internal: a per-env array of the section table is not allocated"); }
   Derived dv;
   derive_model(cfg, d, &dv);
   {  // same derivation one volt higher: the difference is the u_sup-proportional part of the reset observation
@@ -1157,25 +1213,6 @@ int gemb200_set_reference(gemb200_handle* h, const double* ref_in, void* stream)
   return GEMB200_OK;
 }
 
-// checkpoint blob: [header][hot records][cold records][eps][sw][dead-time queue]...  The header pins the blob to the configuration that
-// wrote it: a blob of equal size from another motor / seed / tau / generator set is refused instead of being reinterpreted.
-struct Section { void* ptr; size_t bytes; };
-static int sections(gemb200_handle* h, Section* s) {
-  const size_t n = (size_t)h->cfg.n_envs;
-  int k = 0;
-  s[k++] = {h->d_st, n * (h->NH > 0 ? h->NH : 1) * h->rsz};
-  s[k++] = {h->d_stc, n * h->NC * h->rsz};
-  if (h->d_eps) s[k++] = {h->d_eps, n * sizeof(double)};
-  if (h->d_sw) s[k++] = {h->d_sw, n * sizeof(uint16_t)};
-  if (h->d_fifo) s[k++] = {h->d_fifo, n * h->cfg.dead_time_steps * h->fifo_dim * h->rsz};
-  if (h->d_obsv) s[k++] = {h->d_obsv, n * 4 * h->rsz};
-  if (h->d_sup) s[k++] = {h->d_sup, n * 2 * h->rsz};
-  if (h->d_supph) s[k++] = {h->d_supph, n * sizeof(double)};
-  if (h->d_swst) s[k++] = {h->d_swst, n * 2 * h->cfg.n_ref * sizeof(uint32_t)};
-  if (h->d_kenv) s[k++] = {h->d_kenv, n * sizeof(uint32_t)};
-  if (h->d_imprev) s[k++] = {h->d_imprev, n * 2 * h->rsz};
-  return k;  // (the per-env parameter table is configuration, not state: re-apply gemb200_set_env_params after a load)
-}
 struct CheckpointHeader {
   char magic[8];          // "GEMB200C"
   int32_t abi, dtype, n_envs, n_sections, nh, nc, reserved[2];
@@ -1310,6 +1347,277 @@ int gemb200_kernel_time_end(gemb200_handle* h, void* stream, float* ms_out) {
   CUDA_TRY(cudaEventRecord(h->ev1, (cudaStream_t)stream));
   CUDA_TRY(cudaEventSynchronize(h->ev1));
   CUDA_TRY(cudaEventElapsedTime(ms_out, h->ev0, h->ev1));
+  return GEMB200_OK;
+}
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------------------------
+// Per-env state snapshots (gemb200_pack_envs / gemb200_unpack_envs): packed rows of 32-bit words, format in include/gemb200.h
+// ----------------------------------------------------------------------------------------------------------------
+// The two kernels know nothing about motor families: the section table drives them.  A block of B threads owns B rows.  Each thread moves
+// the arrays of its env to / from its row in shared memory — consecutive threads touch consecutive envs, so the SoA arrays are read and
+// written coalesced, the chunked records with the step kernel's 16-byte accesses — and the block moves its rows to / from global memory
+// word by word, so the [m][words] rows are read and written contiguously as well (the obs row store of the step kernel does the same).
+struct RecSec { char* ptr; int esz, per_env, place, clk, row_off; };
+struct RecArgs {
+  RecSec sec[kMaxSections];
+  int n_sec, n, words, stride;  // sections, envs of the handle, words per row, shared-memory words per row (odd: no bank conflicts)
+  uint32_t div_magic;           // ceil(2^32 / words): row of a block-local word index with one multiply-high
+  int rsz, n_ref, dead, fifo_dim, swst_off;  // swst_off: row word of the switched-generator section, -1 without one
+  int sw_count[kMaxRef], ref_kind[kMaxRefEntries];
+  uint32_t kstep;                // step count (sub-episode clock) and dead-time ring position of the host clock ...
+  int32_t ring;
+  const uint32_t* clock_dev;     // ... or of the device-resident clock (gemb200_set_device_clock), read like clock_of() does
+};
+constexpr int kRecBlockMax = 128;
+
+__device__ __forceinline__ void rec_clock(const RecArgs& a, uint32_t* kstep, int* ring) {
+  if (a.clock_dev) { *kstep = a.clock_dev[2]; *ring = (int)a.clock_dev[3]; }
+  else { *kstep = a.kstep; *ring = a.ring; }
+}
+// element idx of an array of esz-byte elements <-> its row words (two for a double, low word first; a uint16 zero-extended to one)
+template <bool TO_ROW>
+__device__ __forceinline__ void move_elem(char* p, int esz, size_t idx, uint32_t* w) {
+  if (esz == 8) {
+    uint2* q = reinterpret_cast<uint2*>(p) + idx;
+    if (TO_ROW) { const uint2 v = *q; w[0] = v.x; w[1] = v.y; } else *q = make_uint2(w[0], w[1]);
+  } else if (esz == 4) {
+    uint32_t* q = reinterpret_cast<uint32_t*>(p) + idx;
+    if (TO_ROW) w[0] = *q; else *q = w[0];
+  } else {
+    uint16_t* q = reinterpret_cast<uint16_t*>(p) + idx;
+    if (TO_ROW) w[0] = *q; else *q = (uint16_t)w[0];
+  }
+}
+// every section of env i <-> the row; the dead-time ring is rotated so that the row holds it oldest entry first
+template <bool TO_ROW>
+__device__ __forceinline__ void move_env(const RecArgs& a, unsigned i, int ring, uint32_t* row) {
+  const size_t n = (size_t)a.n;
+  for (int s = 0; s < a.n_sec; ++s) {
+    const RecSec& S = a.sec[s];
+    uint32_t* w = row + S.row_off;
+    if (S.place == kRecord) {  // 16-byte chunks, then (fp32) one 8-byte chunk, then one element: gemb200_params.h word_offset()
+      const int vw = 16 / S.esz, nfull = S.per_env / vw, wpe = S.esz / 4;
+      for (int c = 0; c < nfull; ++c) {
+        uint4* q = reinterpret_cast<uint4*>(S.ptr + (size_t)c * 16 * n) + i;
+        uint32_t* d = w + 4 * c;
+        if (TO_ROW) { const uint4 v = *q; d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w; }
+        else *q = make_uint4(d[0], d[1], d[2], d[3]);
+      }
+      int e = nfull * vw;
+      if (vw == 4 && S.per_env - e >= 2) {
+        uint2* q = reinterpret_cast<uint2*>(S.ptr + (size_t)e * 4 * n) + i;
+        uint32_t* d = w + e;
+        if (TO_ROW) { const uint2 v = *q; d[0] = v.x; d[1] = v.y; } else *q = make_uint2(d[0], d[1]);
+        e += 2;
+      }
+      if (e < S.per_env) move_elem<TO_ROW>(S.ptr + (size_t)e * S.esz * n, S.esz, i, w + e * wpe);
+    } else {
+      const int wpe = S.esz == 8 ? 2 : 1;
+      for (int q = 0; q < S.per_env; ++q) {
+        int ae = q;
+        if (S.clk == kClkRing) {  // row entry `slot` (0 = oldest) lives in ring slot (ring + slot) mod dead
+          const int slot = q / a.fifo_dim, j = q - slot * a.fifo_dim;
+          int rs = slot + ring;
+          if (rs >= a.dead) rs -= a.dead;
+          ae = rs * a.fifo_dim + j;
+        }
+        move_elem<TO_ROW>(S.ptr, S.esz, (size_t)ae * n + i, w + q * wpe);
+      }
+    }
+  }
+}
+// a step index kept in a `real` record element (gemb200_kernels.cuh word_to_u32 / u32_to_word): the float's bit pattern, the double's value
+__device__ __forceinline__ uint32_t elem_u32(const uint32_t* w, int rsz) { return rsz == 4 ? w[0] : (uint32_t)__hiloint2double((int)w[1], (int)w[0]); }
+__device__ __forceinline__ void set_elem_u32(uint32_t* w, int rsz, uint32_t u) {
+  if (rsz == 4) { w[0] = u; return; }
+  const double d = (double)u;
+  w[0] = (uint32_t)__double2loint(d); w[1] = (uint32_t)__double2hiint(d);
+}
+// adds `delta` to every clock-relative field of a row: -clock makes them relative (pack), +clock re-bases them (unpack)
+__device__ __forceinline__ void rebase_row(const RecArgs& a, uint32_t* row, uint32_t delta) {
+  for (int s = 0; s < a.n_sec; ++s) {
+    const RecSec& S = a.sec[s];
+    uint32_t* w = row + S.row_off;
+    if (S.clk == kClkCold) {  // cold record [omega | sigma or periodic start per slot | sub-episode end per slot]
+      const int wpe = a.rsz / 4;
+      for (int r = 0; r < a.n_ref; ++r) {
+        uint32_t* end = w + (1 + a.n_ref + r) * wpe;
+        set_elem_u32(end, a.rsz, elem_u32(end, a.rsz) + delta);
+        const unsigned g = (a.sw_count[r] > 1 && a.swst_off >= 0) ? row[a.swst_off + 2 * r] : (unsigned)r;  // the slot's current generator
+        if (g < (unsigned)kMaxRefEntries && a.ref_kind[g] >= GEMB200_REF_SINUS) {
+          uint32_t* start = w + (1 + r) * wpe;
+          set_elem_u32(start, a.rsz, elem_u32(start, a.rsz) + delta);
+        }
+      }
+    } else if (S.clk == kClkSwst) {  // [n_ref][2]: parameter entry, super-episode end
+      for (int r = 0; r < a.n_ref; ++r) w[2 * r + 1] += delta;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kRecBlockMax) pack_envs_kernel(const RecArgs a, const int32_t* __restrict__ env_idx, int m, uint32_t* __restrict__ rows) {
+  extern __shared__ uint32_t srow[];
+  __shared__ int ok[kRecBlockMax];
+  const int t = threadIdx.x, j0 = blockIdx.x * blockDim.x, j = j0 + t;
+  bool valid = false;
+  if (j < m) {
+    const int i = env_idx ? env_idx[j] : j;
+    valid = i >= 0 && i < a.n;
+    if (valid) {
+      uint32_t kstep;
+      int ring;
+      rec_clock(a, &kstep, &ring);
+      uint32_t* row = srow + t * a.stride;
+      move_env<true>(a, (unsigned)i, ring, row);
+      rebase_row(a, row, 0u - kstep);
+    }
+  }
+  ok[t] = valid;
+  __syncthreads();
+  const unsigned total = (unsigned)min((int)blockDim.x, m - j0) * (unsigned)a.words;
+  uint32_t* dst = rows + (size_t)j0 * a.words;
+  for (unsigned k = t; k < total; k += blockDim.x) {
+    const unsigned e = __umulhi(k, a.div_magic), w = k - e * a.words;
+    if (ok[e]) dst[k] = srow[e * a.stride + w];
+  }
+}
+
+__global__ void __launch_bounds__(kRecBlockMax) unpack_envs_kernel(const RecArgs a, const uint32_t* __restrict__ rows, int n_rows, const int32_t* __restrict__ row_idx,
+                                                                  const int32_t* __restrict__ env_idx, int m) {
+  extern __shared__ uint32_t srow[];
+  __shared__ int src[kRecBlockMax];
+  const int t = threadIdx.x, j0 = blockIdx.x * blockDim.x, j = j0 + t;
+  int i = -1, r = -1;
+  if (j < m) {
+    r = row_idx ? row_idx[j] : j;
+    i = env_idx ? env_idx[j] : j;
+    if (r < 0 || r >= n_rows || i < 0 || i >= a.n) r = -1;
+  }
+  src[t] = r;
+  __syncthreads();
+  const unsigned total = (unsigned)min((int)blockDim.x, m - j0) * (unsigned)a.words;
+  for (unsigned k = t; k < total; k += blockDim.x) {
+    const unsigned e = __umulhi(k, a.div_magic), w = k - e * a.words;
+    const int rr = src[e];
+    if (rr >= 0) srow[e * a.stride + w] = __ldg(rows + (size_t)rr * a.words + w);
+  }
+  __syncthreads();
+  if (r >= 0) {
+    uint32_t kstep;
+    int ring;
+    rec_clock(a, &kstep, &ring);
+    uint32_t* row = srow + t * a.stride;
+    rebase_row(a, row, kstep);
+    move_env<false>(a, (unsigned)i, ring, row);
+  }
+}
+
+// FNV-1a over what decides the row format (include/gemb200.h); n_envs, seed, offsets, tau, parameters, reward, ... stay out, so rows move
+// between handles of one env that differ in size or seed
+static uint64_t record_layout_id(const gemb200_config* c, int words) {
+  Dims d;
+  derive_dims(c, &d);
+  uint64_t x = 1469598103934665603ull;
+  auto mix = [&](int64_t v) { for (int b = 0; b < 8; ++b) { x ^= (uint64_t)(v >> (8 * b)) & 0xffu; x *= 1099511628211ull; } };
+  mix(0x47454D5245434F52ll);  // format tag
+  mix(words);
+  mix(c->dtype); mix(c->motor_kind); mix(d.n_ode); mix(c->n_ref);
+  int n_entries = c->n_ref;
+  for (int r = 0; r < c->n_ref; ++r) {
+    const bool sw = c->ref_sw_count[r] > 1;
+    mix(sw ? c->ref_sw_count[r] : 0); mix(sw ? c->ref_sw_first[r] : 0);
+    if (sw && c->ref_sw_first[r] + c->ref_sw_count[r] > n_entries) n_entries = c->ref_sw_first[r] + c->ref_sw_count[r];
+  }
+  for (int e = 0; e < n_entries; ++e) mix(c->ref_kind[e]);
+  mix(has_sw_state(c));
+  mix(c->dead_time_steps); mix(c->dead_time_steps > 0 ? c->dead_time_outer : 0); mix(fifo_dim_of(c, d));
+  mix(c->n_state_ops);
+  for (int k = 0; k < c->n_state_ops; ++k) mix(c->sop_kind[k]);
+  mix(c->supply_kind);
+  mix(c->load_kind == GEMB200_LOAD_EXT_SPEED);
+  mix(c->init_im_valid);
+  return x;
+}
+static int record_words(const gemb200_config* c) {
+  Section s[kMaxSections];
+  const int k = config_sections(c, nullptr, s);
+  int w = 0;
+  for (int q = 0; q < k; ++q) w += row_words(s[q]);
+  return w;
+}
+static void record_args(gemb200_handle* h, RecArgs* a) {
+  std::memset(a, 0, sizeof(*a));
+  Section s[kMaxSections];
+  const int k = sections(h, s);
+  int off = 0;
+  a->swst_off = -1;
+  for (int q = 0; q < k; ++q) {
+    a->sec[q] = {static_cast<char*>(s[q].ptr), s[q].esz, s[q].per_env, s[q].place, s[q].clk, off};
+    if (s[q].clk == kClkSwst) a->swst_off = off;
+    off += row_words(s[q]);
+  }
+  a->n_sec = k; a->n = h->cfg.n_envs; a->words = off; a->stride = off | 1;
+  a->div_magic = (uint32_t)((((uint64_t)1 << 32) + (uint64_t)off - 1) / (uint64_t)off);  // words >= 2: hot and cold record
+  a->rsz = (int)h->rsz; a->n_ref = h->n_ref; a->dead = h->cfg.dead_time_steps; a->fifo_dim = h->fifo_dim;
+  for (int r = 0; r < kMaxRef; ++r) a->sw_count[r] = (r < h->n_ref && h->cfg.ref_sw_count[r] > 1) ? h->cfg.ref_sw_count[r] : 0;
+  for (int e = 0; e < kMaxRefEntries; ++e) a->ref_kind[e] = h->cfg.ref_kind[e];
+  a->kstep = (uint32_t)h->n_steps;
+  a->ring = a->dead > 0 ? (int)(h->n_steps % (uint64_t)a->dead) : 0;
+  a->clock_dev = h->dev_clock ? h->d_clock : nullptr;
+}
+static int record_block(int stride) {  // largest block whose rows fit the default 48 KB of shared memory
+  for (int b = kRecBlockMax; b >= 32; b >>= 1)
+    if ((size_t)b * (size_t)stride * sizeof(uint32_t) <= 48 * 1024) return b;
+  return 0;
+}
+
+extern "C" {
+
+int gemb200_query_env_record(const gemb200_config* cfg, int32_t* words, uint64_t* layout_id) {
+  int rc = validate(cfg);
+  if (rc) return rc;
+  const int w = record_words(cfg);
+  if (words) *words = w;
+  if (layout_id) *layout_id = record_layout_id(cfg, w);
+  return GEMB200_OK;
+}
+
+int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (m < 0) return fail(GEMB200_E_INVALID, "m must be >= 0");
+  if (m == 0) return GEMB200_OK;
+  if (!rows) return fail(GEMB200_E_INVALID, "rows is NULL");
+  DeviceGuard guard(h->cfg.device);
+  RecArgs a;
+  record_args(h, &a);
+  const int block = record_block(a.stride);
+  if (!block) return fail(GEMB200_E_INVALID, "packed env record too long for the shared-memory staging");
+  const int grid = (int)(((int64_t)m + block - 1) / block);
+  pack_envs_kernel<<<grid, block, (size_t)block * a.stride * sizeof(uint32_t), (cudaStream_t)stream>>>(a, env_idx, m, rows);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return GEMB200_OK;
+}
+
+int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
+                        const int32_t* env_idx, int32_t m, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (m < 0 || n_rows < 0) return fail(GEMB200_E_INVALID, "m and n_rows must be >= 0");
+  RecArgs a;
+  record_args(h, &a);
+  if (layout_id != record_layout_id(&h->cfg, a.words))
+    return fail(GEMB200_E_INVALID, "unpack: the rows were packed from a handle with another record layout (motor, dtype, generators, dead time, ...)");
+  if (m == 0 || n_rows == 0) return GEMB200_OK;
+  if (!rows) return fail(GEMB200_E_INVALID, "rows is NULL");
+  DeviceGuard guard(h->cfg.device);
+  const int block = record_block(a.stride);
+  if (!block) return fail(GEMB200_E_INVALID, "packed env record too long for the shared-memory staging");
+  const int grid = (int)(((int64_t)m + block - 1) / block);
+  unpack_envs_kernel<<<grid, block, (size_t)block * a.stride * sizeof(uint32_t), (cudaStream_t)stream>>>(a, rows, n_rows, row_idx, env_idx, m);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
   return GEMB200_OK;
 }
 

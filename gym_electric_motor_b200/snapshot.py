@@ -1,0 +1,70 @@
+"""Per-env state snapshots on the device: the batched counterpart of branching a reference env with `copy.deepcopy(env)`.
+
+An `EnvSnapshot` holds the complete persistent state of m envs as packed rows (gemb200_pack_envs; row format in include/gemb200.h): a
+plain device `torch.int32` tensor [m, words] that the caller may keep, concatenate, index or send to another rank, and that
+`VectorSim.restore` / `ElectricMotorEnvironment.restore_envs` put into any envs of a handle with the same record layout — the same env in
+another batch size, seed or index offset, or with other per-env parameters.  A restored env continues exactly like its source, except
+that it draws the random numbers of its own (seed, global env index) from then on.
+"""
+import numpy as np
+import torch
+
+
+class EnvSnapshot:
+    """Packed state of m envs: `rows` [m, words] int32 on the device, `layout_id` of the record layout, `dtype` of the handle's state.
+    `len(snap)` is m; `snap[k]`, `snap[a:b]`, `snap[index list / tensor]` are sub-snapshots of the selected rows."""
+
+    __slots__ = ("rows", "layout_id", "dtype")
+
+    def __init__(self, rows, layout_id, dtype):
+        if not isinstance(rows, torch.Tensor) or rows.dtype != torch.int32 or rows.dim() != 2:
+            raise ValueError("EnvSnapshot rows must be a 2-D torch.int32 tensor [m, words]")
+        self.rows = rows
+        self.layout_id = int(layout_id)
+        self.dtype = dtype
+
+    def __len__(self):
+        return int(self.rows.shape[0])
+
+    @property
+    def words(self):
+        return int(self.rows.shape[1])
+
+    def __getitem__(self, idx):
+        if isinstance(idx, (int, np.integer)):
+            k = int(idx) + (len(self) if int(idx) < 0 else 0)
+            if not 0 <= k < len(self):
+                raise IndexError(f"snapshot index {idx} out of range for {len(self)} rows")
+            sub = self.rows[k:k + 1]
+        elif isinstance(idx, slice):
+            sub = self.rows[idx]
+        else:
+            sub = self.rows[torch.as_tensor(np.asarray(idx) if not isinstance(idx, torch.Tensor) else idx, device=self.rows.device).long()]
+        return EnvSnapshot(sub.contiguous(), self.layout_id, self.dtype)
+
+    def __repr__(self):
+        return f"EnvSnapshot(m={len(self)}, words={self.words}, layout_id={self.layout_id:#018x}, dtype={self.dtype})"
+
+
+def check_host_index(idx, bound, what):
+    """Range check of a host-side index argument (list, numpy array, CPU tensor): IndexError unless every entry is in [0, bound).
+    None and device tensors pass unchanged (the kernels skip out-of-range entries of a device index)."""
+    if idx is None or (isinstance(idx, torch.Tensor) and idx.is_cuda):
+        return idx
+    a = np.asarray(idx.cpu() if isinstance(idx, torch.Tensor) else idx).reshape(-1)
+    if a.size and not np.issubdtype(a.dtype, np.integer):
+        raise IndexError(f"{what} must hold integers, got {a.dtype}")
+    if a.size and (a.min() < 0 or a.max() >= bound):
+        raise IndexError(f"{what} out of range: entries must be in [0, {bound})")
+    return a
+
+
+def check_layout(snap, words, layout_id):
+    """ValueError unless `snap` was packed from a handle with this record layout"""
+    if not isinstance(snap, EnvSnapshot):
+        raise ValueError(f"expected an EnvSnapshot, got {type(snap).__name__}")
+    if snap.layout_id != int(layout_id):
+        raise ValueError(f"snapshot of another record layout (layout_id {snap.layout_id:#018x}, this env has {int(layout_id):#018x}): "
+                         "motor, dtype, generators, dead time, wrappers or supply differ")
+    if snap.words != int(words):
+        raise ValueError(f"snapshot rows have {snap.words} words, this env's record has {int(words)}")

@@ -237,6 +237,51 @@ class VectorSim:
             raise ValueError("checkpoint size mismatch")
         K.check(self._lib.gemb200_checkpoint_load(self._h, buf.ctypes.data_as(C.c_void_p)), "gemb200_checkpoint_load")
 
+    # ------------------------------------------------------------------ per-env snapshots (snapshot.py)
+    def record_layout(self):
+        """(words per env of a packed record, layout id) of this handle's configuration (gemb200_query_env_record)"""
+        if getattr(self, "_record", None) is None:
+            w, lid = C.c_int32(), C.c_uint64()
+            K.check(self._lib.gemb200_query_env_record(C.byref(self.cfg), C.byref(w), C.byref(lid)), "gemb200_query_env_record")
+            self._record = (int(w.value), int(lid.value))
+        return self._record
+
+    def _dev_index(self, idx):
+        if idx is None:
+            return None
+        t = idx if isinstance(idx, torch.Tensor) else torch.as_tensor(np.asarray(idx, dtype=np.int64).reshape(-1))
+        return t.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
+
+    def snapshot(self, idx=None):
+        """Pack the persistent state of envs `idx` (None: all) into an EnvSnapshot (gemb200_pack_envs; stream-ordered, no host sync).
+        Row j holds env idx[j]; a device index entry out of range leaves its row uninitialised."""
+        from .snapshot import EnvSnapshot
+
+        words, lid = self.record_layout()
+        ii = self._dev_index(idx)
+        m = self.n if ii is None else int(ii.numel())
+        rows = torch.empty((m, words), dtype=torch.int32, device=self.device)
+        K.check(self._lib.gemb200_pack_envs(self._h, _ptr(ii), m, _ptr(rows), self._stream()), "gemb200_pack_envs")
+        return EnvSnapshot(rows, lid, self.dtype)
+
+    def restore(self, snap, idx=None, rows=None):
+        """Env idx[j] (None: j) takes the state of snapshot row rows[j] (None: j) (gemb200_unpack_envs; stream-ordered, no host sync).
+        `rows` fans one snapshot out: restore(snap, idx=range(C * m), rows=np.repeat(range(m), C)) copies every row into C envs.
+        Device index entries out of range are skipped."""
+        from .snapshot import check_layout
+
+        words, lid = self.record_layout()
+        check_layout(snap, words, lid)
+        ii, rr = self._dev_index(idx), self._dev_index(rows)
+        if ii is not None and rr is not None and ii.numel() != rr.numel():
+            raise ValueError(f"idx ({ii.numel()}) and rows ({rr.numel()}) must have the same length")
+        m = int(ii.numel()) if ii is not None else (int(rr.numel()) if rr is not None else min(len(snap), self.n))
+        if snap.rows.device != self.device:
+            raise ValueError(f"snapshot rows are on {snap.rows.device}, this handle on {self.device}: move the rows first")
+        data = snap.rows.contiguous()
+        K.check(self._lib.gemb200_unpack_envs(self._h, _ptr(data), len(snap), C.c_uint64(lid), _ptr(rr), _ptr(ii), m, self._stream()),
+                "gemb200_unpack_envs")
+
     # ------------------------------------------------------------------ measurement helpers
     @property
     def launch_count(self):

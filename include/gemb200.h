@@ -373,6 +373,44 @@ int64_t gemb200_checkpoint_size(gemb200_handle* h);
 int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob);
 int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob);
 
+/* Per-env state snapshots on the device (the batched counterpart of copy.deepcopy(env) in the reference): branch, archive and fan out
+ * environments without a host round trip.  gemb200_pack_envs copies the complete persistent state of chosen envs into packed rows,
+ * gemb200_unpack_envs puts rows into chosen envs of any handle of the same record layout (a plant handle of N envs can seed a model handle
+ * of N*C envs; n_envs, seed, env_index_offset, tau, solver, parameters, limits, reward, constraints and I/O layout may all differ).
+ * All pointers are device pointers; both calls are stream-ordered, never synchronise the host and can be captured in a CUDA graph (with
+ * the device clock on they read the step count and the dead-time ring position from device memory).  Entries of env_idx / row_idx that
+ * are out of range are skipped (pack leaves that row untouched).  Two entries of env_idx naming the same env in one unpack race.
+ *
+ * Row format: `words` 32-bit words per env, the persistent per-env arrays of the handle in the checkpoint's section order, each copied as
+ * raw words (fp64 values as two words, low word first; a uint16 switching state zero-extended to one word):
+ *   hot record [hot_words]   x_1..x_{nx-1}, reference value per slot                              (real)
+ *   cold record [cold_words] omega, sigma or periodic start step per slot, sub-episode end per slot (real)
+ *   angle                    double (DC motors: absent)
+ *   finite switching state   uint16 -> 1 word (finite converters with interlocking time or an RC supply)
+ *   dead-time queue          [dead_time_steps][fifo_dim] real, OLDEST entry first
+ *   FluxObserver integrator  [4] real
+ *   RC supply                [2] real
+ *   AC supply phase          double
+ *   switched generators      [n_ref][2] uint32: parameter entry, super-episode end
+ *   external-profile clock   uint32 steps since the reset
+ *   im_prev                  [2] real (induction motors with random initial states)
+ * Fields kept against the handle's step count are stored RELATIVE to it (u32 difference, the same u32 encoding the record uses: the float
+ * bit pattern in fp32, the integral double value in fp64): the sub-episode ends, the start step of a slot whose current generator is
+ * periodic (sinus / step / sawtooth / triangular), and the super-episode ends.  Unpack re-bases them on the destination's step count.
+ * Not in the row: the per-env parameter table (configuration, like in the checkpoint) and the RNG identity — a restored env draws the
+ * random numbers of ITS OWN (seed, global index) from then on.
+ * layout_id: FNV-1a over what decides the row format (dtype, motor, n_ode, n_ref, generator kinds and switched grouping, switching-state
+ * array, dead time and its order and queue width, state-op kinds, supply, external speed load, induction motor with random initial
+ * states); not over n_envs, seed, offsets, device, tau, solver, parameters, limits, reward, constraints, autoreset or layout. */
+/* words per env of a packed record and the id of its layout; no GPU needed (like gemb200_query_dims) */
+int gemb200_query_env_record(const gemb200_config* cfg, int32_t* words, uint64_t* layout_id);
+/* rows[j][0..words) = packed state of env env_idx[j] (env_idx NULL: env j), j < m */
+int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream);
+/* env env_idx[j] (NULL: j) takes the state in rows[row_idx[j]] (NULL: row j), j < m; row_idx entries index [0, n_rows); refuses rows
+ * of another layout_id with GEMB200_E_INVALID */
+int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
+                        const int32_t* env_idx, int32_t m, void* stream);
+
 /* Introspection used by bench.py: number of kernel launches issued through this handle so far, and the
  * CUDA-event time in ms of the step launches since the last call (see DESIGN.md "Measurement"). */
 int64_t gemb200_launch_count(gemb200_handle* h);

@@ -1,0 +1,146 @@
+"""Per-env snapshot throughput (gemb200_pack_envs / gemb200_unpack_envs) and a random-shooting MPC control step built on it.
+
+    python tools/branch_bench.py [--envs 1048576] [--reps 20]
+
+Prints the GPU name and power limit, then one JSON line per measurement (CUDA events, median over --reps):
+  1. pack and unpack of all envs of Cont-CC-PMSM-v0 (fp32: 11 words = 44 B per env), bytes moved and the fraction of the H100 SXM data-sheet
+     bandwidth (3.35 TB/s);
+  2. fan-out unpack of 1024 rows into all envs (row_idx: every row into envs/1024 consecutive envs);
+  3. a random-shooting MPC control step, 1024 plants x 1024 candidates x horizon 8: pack the plants, fan them out into the model handle,
+     rollout recording only the rewards, sum over the horizon, argmax per plant, step the plants with the first action of their best
+     branch.  The candidate actions are drawn once up front (their generation is the policy's cost, not the simulator's).
+Run from the repository root after the build; writes nothing.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+
+import gym_electric_motor_b200 as gem  # noqa: E402
+from gym_electric_motor_b200.vector_sim import VectorSim  # noqa: E402
+
+PEAK = 3.35e12  # H100 SXM data-sheet HBM3 bandwidth, B/s
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
+                             timeout=20).stdout.strip()
+        name, plimit = [x.strip() for x in out.split(",")[:2]]
+        return name, plimit
+    except Exception:  # noqa: BLE001
+        return torch.cuda.get_device_name(0), "unknown"
+
+
+def timed(fn, reps, warmup=3):
+    for _ in range(warmup):
+        fn()
+    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
+    for a, b in ev:
+        a.record()
+        fn()
+        b.record()
+    torch.cuda.synchronize()
+    ms = sorted(a.elapsed_time(b) for a, b in ev)
+    return ms[len(ms) // 2]
+
+
+def sim_of(n, seed=0):
+    env = gem.make("Cont-CC-PMSM-v0", num_envs=n)
+    cfg = env.build_config()
+    cfg.seed = seed
+    return VectorSim(cfg)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--envs", type=int, default=1 << 20)
+    ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--plants", type=int, default=1024)
+    ap.add_argument("--horizon", type=int, default=8)
+    args = ap.parse_args()
+    name, plimit = gpu_info()
+    print(f"GPU: {name}, power limit {plimit}")
+    n = args.envs
+    sim = sim_of(n)
+    sim.reset()
+    words, _ = sim.record_layout()
+    rec_bytes = 4 * words
+    snap = sim.snapshot()
+    torch.cuda.synchronize()
+
+    ms = timed(lambda: sim.snapshot(), args.reps)
+    moved = 2 * rec_bytes * n  # state read + rows written
+    print(json.dumps(dict(what="pack", envs=n, words=words, ms=round(ms, 4), bytes=moved, tb_s=round(moved / ms / 1e9, 3),
+                          frac_datasheet=round(moved / ms / 1e-3 / PEAK, 3))))
+    ms = timed(lambda: sim.restore(snap), args.reps)
+    print(json.dumps(dict(what="unpack", envs=n, words=words, ms=round(ms, 4), bytes=moved, tb_s=round(moved / ms / 1e9, 3),
+                          frac_datasheet=round(moved / ms / 1e-3 / PEAK, 3))))
+
+    m = 1024
+    few = snap[:m]
+    ridx = torch.arange(m, device=sim.device, dtype=torch.int32).repeat_interleave(n // m)
+    ms = timed(lambda: sim.restore(few, rows=ridx), args.reps)
+    moved_f = (rec_bytes + 4) * n + rec_bytes * m  # state written + row index read + the (L2-resident) rows once
+    print(json.dumps(dict(what="fan_out_unpack", rows=m, envs=n, ms=round(ms, 4), bytes=moved_f, tb_s=round(moved_f / ms / 1e9, 3),
+                          frac_datasheet=round(moved_f / ms / 1e-3 / PEAK, 3))))
+    del sim, snap, few
+
+    # random-shooting MPC: P plants x C candidates x horizon H
+    p_n, h = args.plants, args.horizon
+    c = n // p_n
+    plant, model = sim_of(p_n, seed=1), sim_of(p_n * c, seed=2)
+    plant.reset()
+    model.reset()
+    gen = torch.Generator(device=plant.device).manual_seed(0)
+    cand = (torch.rand((h, p_n * c, model.n_act), device=plant.device, generator=gen) * 2 - 1).contiguous()
+    rew = torch.empty((h, p_n * c), dtype=model.dtype, device=plant.device)
+    ridx = torch.arange(p_n, device=plant.device, dtype=torch.int32).repeat_interleave(c)
+    base = torch.arange(p_n, device=plant.device) * c
+    marks = []
+
+    def control_step(record=False):
+        e = [torch.cuda.Event(enable_timing=True) for _ in range(6)] if record else None
+        if record:
+            e[0].record()
+        s = plant.snapshot()
+        if record:
+            e[1].record()
+        model.restore(s, rows=ridx)
+        if record:
+            e[2].record()
+        model.rollout_into(cand, h, 1, None, None, rew, None)
+        if record:
+            e[3].record()
+        best = rew.sum(0).view(p_n, c).argmax(1) + base
+        act = cand[0].index_select(0, best)
+        if record:
+            e[4].record()
+        plant.step(act)
+        if record:
+            e[5].record()
+            marks.append(e)
+
+    for _ in range(3):
+        control_step()
+    torch.cuda.synchronize()
+    for _ in range(args.reps):
+        control_step(record=True)
+    torch.cuda.synchronize()
+    split = {}
+    for k, lab in enumerate(["pack", "fan_out", "rollout", "select", "plant_step"]):
+        v = sorted(e[k].elapsed_time(e[k + 1]) for e in marks)
+        split[lab] = round(v[len(v) // 2], 4)
+    tot = sorted(e[0].elapsed_time(e[5]) for e in marks)
+    tot_ms = tot[len(tot) // 2]
+    print(json.dumps(dict(what="mpc_control_step", plants=p_n, candidates=c, horizon=h, ms=round(tot_ms, 4), control_steps_per_s=round(1e3 / tot_ms, 1),
+                          env_steps_per_s=round(p_n * c * h / tot_ms * 1e3, 1), split_ms=split)))
+
+
+if __name__ == "__main__":
+    main()
