@@ -27,6 +27,8 @@ AUTORESET_NONE, AUTORESET_SAME_STEP = 0, 1
 SOP_NONE, SOP_COS_SIN, SOP_FLUX_OBSERVER, SOP_NOISE, SOP_CURRENT_SUM = range(5)
 NOISE_NORMAL, NOISE_UNIFORM, NOISE_LAPLACE = range(3)
 SUPPLY_IDEAL, SUPPLY_RC, SUPPLY_AC1 = 0, 1, 2
+DIST_UNIFORM, DIST_LOG_UNIFORM = 0, 1
+MAX_DRAW = MAX_MOTOR_PARAM + 8  # parameter slots of gemb200_set_param_randomization: motor slots, then load slots
 
 E_INVALID, E_CUDA, E_NOMEM, E_ABI = -1, -2, -3, -4
 
@@ -146,7 +148,7 @@ SYMBOLS = [
     "gemb200_get_ode_state", "gemb200_set_ode_state", "gemb200_get_reference", "gemb200_set_reference",
     "gemb200_reseed", "gemb200_set_device_clock", "gemb200_get_clock", "gemb200_set_env_params", "gemb200_peer_buffer_alloc", "gemb200_peer_buffer_open", "gemb200_peer_buffer_close",
     "gemb200_peer_buffer_free", "gemb200_bind_peers", "gemb200_peer_signal", "gemb200_peer_wait", "gemb200_checkpoint_size", "gemb200_checkpoint_save", "gemb200_checkpoint_load", "gemb200_query_env_record",
-    "gemb200_pack_envs", "gemb200_unpack_envs", "gemb200_launch_count",
+    "gemb200_pack_envs", "gemb200_unpack_envs", "gemb200_set_param_randomization", "gemb200_get_env_params", "gemb200_launch_count",
     "gemb200_kernel_time_begin", "gemb200_kernel_time_end",
 ]
 
@@ -197,6 +199,8 @@ def load_library():
     lib.gemb200_set_device_clock.argtypes = [vp, C.c_int32, vp]
     lib.gemb200_get_clock.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), vp]
     lib.gemb200_set_env_params.argtypes = [vp, vp, vp]
+    lib.gemb200_set_param_randomization.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
+    lib.gemb200_get_env_params.argtypes = [vp, vp, vp]
     lib.gemb200_peer_buffer_alloc.argtypes = [C.c_int32, C.c_int64, C.POINTER(vp), vp]
     lib.gemb200_peer_buffer_open.argtypes = [C.c_int32, vp, C.POINTER(vp)]
     lib.gemb200_peer_buffer_close.argtypes = [C.c_int32, vp]

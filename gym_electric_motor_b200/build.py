@@ -14,7 +14,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 HEADERS = [os.path.join(CSRC, "gemb200_kernels.cuh"), os.path.join(CSRC, "gemb200_params.h"), os.path.join(CSRC, "gemb200_launch.cuh"),
-           os.path.join(HERE, "..", "include", "gemb200.h")]
+           os.path.join(CSRC, "gemb200_model.h"), os.path.join(HERE, "..", "include", "gemb200.h")]
 SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu")]
 OUT = os.path.join(HERE, "libgemb200.so")
 OBJ_DIR = os.path.join(HERE, "..", "build", "gemb200")

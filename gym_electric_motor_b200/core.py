@@ -323,6 +323,38 @@ class ElectricMotorEnvironment(_EnvBase):
             lp[:, self._LP_SLOT[name]] = np.broadcast_to(np.asarray(vals, dtype=np.float64), (sim.n,))
         sim.set_env_params(mp, lp)
 
+    def randomize_env_parameters(self, motor_parameter=None, load_parameter=None):
+        """Per-episode domain randomisation: from now on EVERY reset of an env — `reset()`, with or without a mask, and the in-kernel
+        auto-reset of `step`, `rollout` and captured graphs — draws new values for the named parameters from the env's own random stream.
+        Both arguments are dicts  name -> distribution  with the names of `set_env_parameters`; a distribution is `(lo, hi)` (uniform) or
+        `("uniform" | "log_uniform", lo, hi)`.  A drawn value is rounded to the env's dtype; the new episode's dynamics and its reset
+        observation use it.  Parameters that are not named keep their current value.  Draws are reproducible: equal seeds give equal
+        sequences, independent of sharding.  The call itself draws nothing (the usual pattern is this call, then `reset()`);
+        `randomize_env_parameters()` without arguments stops drawing and the envs keep their last values.  Pole pairs cannot be drawn
+        (ValueError); nor, for induction motors with random initial states, the parameters of their flux limits (NotImplementedError).
+        Needs the row-per-env (AoS) layout (ValueError).  While draws are on, checkpoints and snapshots are refused (DESIGN.md §7)."""
+        if self._scalar:
+            raise TypeError("randomize_env_parameters() needs a batched environment (num_envs=...)")
+        from .randomization import encode_distributions
+
+        cfg = self._sim.cfg if self._sim is not None else self.build_config()
+        if cfg.layout == K.LAYOUT_SOA and (motor_parameter or load_parameter):
+            raise ValueError("per-env parameter draws need the row-per-env layout (layout='aos')")
+        names, slots, kinds, lo, hi = encode_distributions(motor_parameter, load_parameter, self._MP_SLOT, self._LP_SLOT,
+                                                           flux_limits=bool(cfg.init_im_valid))
+        self._ensure_sim().set_param_randomization(slots, kinds, lo, hi)
+        self._randomized_names = tuple(names)
+
+    _randomized_names = ()
+
+    def env_parameters(self):
+        """{name: tensor[N]} on the device: the stored values (env dtype) of the parameters drawn at every reset."""
+        sim = self._ensure_sim()
+        if not sim.randomized_slots:
+            return {}
+        vals = sim.env_params()
+        return {name: vals[j] for j, name in enumerate(self._randomized_names)}
+
     def snapshot_envs(self, idx=None):
         """Branching support, the batched counterpart of `copy.deepcopy(env)`: the complete persistent state of envs `idx` (None: all;
         list, numpy array or tensor) as an `EnvSnapshot` of packed device rows, taken without a host synchronisation.  Host-side

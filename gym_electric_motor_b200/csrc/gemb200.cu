@@ -50,6 +50,9 @@ struct gemb200_handle {
   void* d_obsv = nullptr;  // FluxObserver integrator [4][n]: re, im, compensation of re, of im
   void* d_envp = nullptr;    // per-env model coefficients [kCoefWords][n] (gemb200_set_env_params), nullptr: shared coefficients
   int plain_shape = 0;       // the configuration has the PLAIN shape (before per-env parameters switch the specialisation off)
+  double* d_praw = nullptr;  // physical parameters per env [kMaxDraw][n] (double), valid whenever d_envp is in use
+  ParamDraw* d_draw = nullptr;  // distributions of the parameters drawn at every reset (gemb200_set_param_randomization)
+  int n_draw = 0;               // parameters drawn per reset (0: none)
   void* d_imprev = nullptr;  // induction motors with random initial states [2][n]: initial currents of the env's previous episode
   int n_obs = 0, row_stride = 0;
   StepParams<float> pf;
@@ -269,7 +272,8 @@ static int config_sections(const gemb200_config* c, const gemb200_handle* h, Sec
   if (any_switched_slot(c)) add(h ? h->d_swst : nullptr, 4, 2 * c->n_ref, kPlanar, kClkSwst);
   if (c->load_kind == GEMB200_LOAD_EXT_SPEED) add(h ? h->d_kenv : nullptr, 4, 1, kPlanar, kClkNone);
   if (c->init_im_valid) add(h ? h->d_imprev : nullptr, rsz, 2, kPlanar, kClkNone);
-  return k;  // (the per-env parameter table is configuration, not state: re-apply gemb200_set_env_params after a load)
+  return k;  // (the per-env parameter table is configuration, not state: re-apply gemb200_set_env_params after a load; parameter draws
+             //  per reset make it state, so checkpoints and snapshots are refused while they are on)
 }
 static int sections(gemb200_handle* h, Section* s) { return config_sections(&h->cfg, h, s); }
 static bool sections_allocated(gemb200_handle* h) {
@@ -292,65 +296,11 @@ struct Derived {
 };
 
 static void derive_model(const gemb200_config* cfg, const Dims& dm, Derived* o) {
-  const double* mp = cfg->motor_param;
-  const double p = mp[GEMB200_MP_P], r_s = mp[GEMB200_MP_R_S], l_d = mp[GEMB200_MP_L_D], l_q = mp[GEMB200_MP_L_Q];
-  double* c = o->c;
-  switch (cfg->motor_kind) {
-    case GEMB200_MOTOR_PERMEX_DC: {  // dc_permanently_excited_motor.py:71-75
-      const double l_a = mp[GEMB200_MP_L_A];
-      c[0] = -mp[GEMB200_MP_PSI_E] / l_a; c[1] = -mp[GEMB200_MP_R_A] / l_a; c[2] = 0; c[3] = 1.0 / l_a;
-      o->tq[0] = mp[GEMB200_MP_PSI_E]; o->tq[1] = 0;
-    } break;
-    case GEMB200_MOTOR_SERIES_DC: {  // dc_series_motor.py:66-74
-      const double l = mp[GEMB200_MP_L_A] + mp[GEMB200_MP_L_E];
-      c[0] = 0; c[1] = (-mp[GEMB200_MP_R_A] - mp[GEMB200_MP_R_E]) / l; c[2] = -mp[GEMB200_MP_L_E_PRIME] / l; c[3] = 1.0 / l;
-      o->tq[0] = 0; o->tq[1] = mp[GEMB200_MP_L_E_PRIME];
-    } break;
-    case GEMB200_MOTOR_SHUNT_DC:
-    case GEMB200_MOTOR_EXTEX_DC: {  // dc_motor.py:95-108
-      const double l_a = mp[GEMB200_MP_L_A], l_e = mp[GEMB200_MP_L_E];
-      c[0] = -mp[GEMB200_MP_R_A] / l_a; c[1] = -mp[GEMB200_MP_L_E_PRIME] / l_a; c[2] = 1.0 / l_a;
-      c[3] = -mp[GEMB200_MP_R_E] / l_e; c[4] = 1.0 / l_e;
-      o->tq[0] = mp[GEMB200_MP_L_E_PRIME];
-    } break;
-    case GEMB200_MOTOR_PMSM:
-    case GEMB200_MOTOR_SYNRM: {  // permanent_magnet_synchronous_motor.py:107-139, synchronous_reluctance_motor.py:117-139
-      const double psi_p = cfg->motor_kind == GEMB200_MOTOR_PMSM ? mp[GEMB200_MP_PSI_P] : 0.0;
-      c[0] = -r_s / l_d; c[1] = 1.0 / l_d; c[2] = l_q * p / l_d;
-      c[3] = -psi_p * p / l_q; c[4] = -r_s / l_q; c[5] = 1.0 / l_q; c[6] = -l_d * p / l_q;
-      o->tq[0] = 1.5 * p * psi_p; o->tq[1] = 1.5 * p * (l_d - l_q);
-    } break;
-    case GEMB200_MOTOR_EESM: {  // externally_excited_synchronous_motor.py:125-153, :200-203
-      const double k = mp[GEMB200_MP_K], r_e = mp[GEMB200_MP_R_E], l_m = mp[GEMB200_MP_L_M], l_e = mp[GEMB200_MP_L_E];
-      const double r_E = k * k * 1.5 * r_e, l_M = k * 1.5 * l_m, l_E = k * k * 1.5 * l_e, ik = 2.0 / 3.0 / k;
-      const double sigma = 1.0 - l_M * l_M / (l_d * l_E);
-      c[0] = (-r_s / sigma) / l_d; c[1] = (l_M * r_E / (sigma * l_E) * ik) / l_d; c[2] = (1.0 / sigma) / l_d;
-      c[3] = (-l_M * k / (sigma * l_E)) / l_d; c[4] = (l_q * p / sigma) / l_d;
-      c[5] = -r_s / l_q; c[6] = 1.0 / l_q; c[7] = -l_d * p / l_q; c[8] = -p * l_M * ik / l_q;
-      const double s2 = l_E * ik;
-      c[9] = (l_M * r_s / (sigma * l_d)) / s2; c[10] = (-r_E / sigma * ik) / s2; c[11] = (-l_M / (sigma * l_d)) / s2;
-      c[12] = (k / sigma) / s2; c[13] = (-p * l_M * l_q / (sigma * l_d)) / s2;
-      o->tq[0] = 1.5 * p * l_M * ik; o->tq[1] = 1.5 * p * (l_d - l_q);
-    } break;
-    case GEMB200_MOTOR_DFIM:
-    case GEMB200_MOTOR_SCIM: {  // induction_motor.py:287-310, :236-249
-      const double l_m = mp[GEMB200_MP_L_M], r_r = mp[GEMB200_MP_R_E];
-      const double l_s = l_m + mp[GEMB200_MP_L_SIGS], l_r = l_m + mp[GEMB200_MP_L_SIGR];
-      const double sigma = (l_s * l_r - l_m * l_m) / (l_s * l_r);
-      const double tau_r = l_r / r_r, tau_sig = sigma * l_s / (r_s + r_r * (l_m * l_m) / (l_r * l_r));
-      c[0] = -1.0 / tau_sig; c[1] = l_m * r_r / (sigma * l_s * l_r * l_r); c[2] = l_m * p / (sigma * l_r * l_s);
-      c[3] = 1.0 / (sigma * l_s); c[4] = l_m / tau_r; c[5] = -1.0 / tau_r; c[6] = p;
-      c[7] = -l_m / (sigma * l_r * l_s);  // rotor-voltage column of the current rows (DFIM)
-      c[8] = 1.0 / l_r; c[9] = l_m / l_r;  // rotor current i_r = psi_r / l_r - l_m / l_r * i_s (physical_systems.py:946-956)
-      o->tq[0] = 1.5 * p * l_m / l_r;
-    } break;
-  }
-  // MechanicalLoad.set_j_rotor mechanical_load.py:188-193, polynomial_static_load.py:60-64
-  const double* lp = cfg->load_param;
-  const double j_total = lp[GEMB200_LP_J_LOAD] + mp[GEMB200_MP_J_ROTOR];
-  o->inv_j = j_total > 0 ? 1.0 / j_total : 0.0;
-  o->omega_lin = j_total / lp[GEMB200_LP_TAU_DECAY];
-  o->omega_lim = j_total > 0 ? lp[GEMB200_LP_A] / j_total * lp[GEMB200_LP_TAU_DECAY] : 0.0;
+  ModelCoef mc;
+  derive_coef(cfg->motor_kind, cfg->motor_param, cfg->load_param, &mc);  // gemb200_model.h: shared with the parameter draws on the device
+  for (int j = 0; j < 20; ++j) o->c[j] = mc.c[j];
+  for (int j = 0; j < 4; ++j) o->tq[j] = mc.tq[j];
+  o->inv_j = mc.inv_j; o->omega_lim = mc.omega_lim; o->omega_lin = mc.omega_lin;
 
   // observation right after reset (SCMLSystem.reset physical_systems.py:256-287, :527-561, :659-693, :816-847) for the
   // constant initial state; converter.reset() gives 0 per QC and -0.5 per B6 leg (converters.py:45-54, :880-886)
@@ -928,6 +878,7 @@ int gemb200_destroy(gemb200_handle* h) {
   if (!h) return GEMB200_OK;
   DeviceGuard guard(h->cfg.device);
   cudaFree(h->d_st); cudaFree(h->d_stc); cudaFree(h->d_eps); cudaFree(h->d_sw); cudaFree(h->d_fifo); cudaFree(h->d_obsv); cudaFree(h->d_sup); cudaFree(h->d_supph); cudaFree(h->d_swst); cudaFree(h->d_ext); cudaFree(h->d_kenv); cudaFree(h->d_imprev); cudaFree(h->d_envp); cudaFree(h->d_clock);
+  cudaFree(h->d_praw); cudaFree(h->d_draw);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_ref); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_mask);
   if (h->hstream) cudaStreamDestroy(h->hstream);
   for (int k = 0; k < 3; ++k) if (h->hpipe[k]) cudaStreamDestroy(h->hpipe[k]);
@@ -975,6 +926,7 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
     return fail(GEMB200_E_INVALID, "per-env parameter blocks need the row-per-env (AoS) I/O layout");
   if (!motor_param && !load_param) {
     h->pf.envp = nullptr; h->pd.envp = nullptr;
+    h->n_draw = 0; h->pf.n_draw = 0; h->pd.n_draw = 0;  // shared coefficients again: no parameter draws either
     h->pf.plain = h->pf.n_dst == 0 ? h->plain_shape : 0; h->pd.plain = h->pf.plain;
     return GEMB200_OK;
   }
@@ -982,10 +934,13 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   Dims d;
   derive_dims(&h->cfg, &d);
   std::vector<double> tab((size_t)kCoefWords * n);
+  std::vector<double> raw((size_t)kMaxDraw * n);  // the physical parameters themselves: what parameter draws at a reset start from
   gemb200_config c = h->cfg;
   for (size_t i = 0; i < n; ++i) {
     if (motor_param) std::memcpy(c.motor_param, motor_param + i * GEMB200_MAX_MOTOR_PARAM, sizeof(c.motor_param));
     if (load_param) std::memcpy(c.load_param, load_param + i * 8, sizeof(c.load_param));
+    for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw[(size_t)s * n + i] = c.motor_param[s];
+    for (int s = 0; s < 8; ++s) raw[(size_t)(GEMB200_MAX_MOTOR_PARAM + s) * n + i] = c.load_param[s];
     if (c.load_kind == GEMB200_LOAD_POLY_STATIC && !(c.load_param[GEMB200_LP_J_LOAD] + c.motor_param[GEMB200_MP_J_ROTOR] > 0))
       return fail(GEMB200_E_INVALID, "per-env parameters: total inertia must be positive for every env");
     Derived dv;
@@ -997,6 +952,8 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   }
   for (double v : tab) if (!std::isfinite(v)) return fail(GEMB200_E_INVALID, "per-env parameters: a derived model coefficient is not finite (zero inductance?)");
   if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, tab.size() * h->rsz));
+  if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, raw.size() * sizeof(double)));
+  CUDA_TRY(cudaMemcpy(h->d_praw, raw.data(), raw.size() * sizeof(double), cudaMemcpyHostToDevice));
   if (h->cfg.dtype == GEMB200_F32) {
     std::vector<float> tf(tab.begin(), tab.end());
     CUDA_TRY(cudaMemcpy(h->d_envp, tf.data(), tf.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -1005,6 +962,99 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   }
   h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
   h->pf.plain = 0; h->pd.plain = 0;  // the PLAIN instantiations read the shared constant-bank coefficients
+  h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
+  return GEMB200_OK;
+}
+
+}  // extern "C"
+
+// Per-env parameter blocks filled on the device from the shared configuration: every env gets the shared coefficients (the values
+// gemb200_set_env_params derives from rows equal to the configuration's) and the configuration's physical parameters.
+struct RawParams { double v[kMaxDraw]; };
+template <typename real>
+__global__ void fill_env_params_kernel(real* envp, double* praw, const Coef<real> k, const RawParams raw, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const size_t nn = (size_t)n;
+  for (int w = 0; w < 20; ++w) envp[w * nn + i] = k.c[w];
+  for (int w = 0; w < 4; ++w) envp[(20 + w) * nn + i] = k.tq[w];
+  envp[24 * nn + i] = k.load_a; envp[25 * nn + i] = k.load_b; envp[26 * nn + i] = k.load_c;
+  envp[27 * nn + i] = k.inv_j; envp[28 * nn + i] = k.omega_lim; envp[29 * nn + i] = k.omega_lin;
+  for (int s = 0; s < kMaxDraw; ++s) praw[s * nn + i] = raw.v[s];
+}
+// out[j][i] = stored value of drawn parameter j of env i, in the handle's dtype
+template <typename real>
+__global__ void get_env_params_kernel(const double* praw, const ParamDraw* d, int n_draw, real* out, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (int j = 0; j < n_draw; ++j) out[(size_t)j * n + i] = (real)praw[(size_t)d->slot[j] * n + i];
+}
+
+extern "C" {
+
+int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t* slot, const int32_t* kind, const double* lo, const double* hi) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (n < 0 || n > kMaxDraw) return fail(GEMB200_E_INVALID, "number of drawn parameters out of range");
+  if (n > 0 && (!slot || !kind || !lo || !hi)) return fail(GEMB200_E_INVALID, "NULL argument");
+  DeviceGuard guard(h->cfg.device);
+  CUDA_TRY(cudaDeviceSynchronize());
+  if (n == 0) {  // no more draws; the envs keep their last values
+    h->n_draw = 0; h->pf.n_draw = 0; h->pd.n_draw = 0;
+    return GEMB200_OK;
+  }
+  if (h->cfg.layout != GEMB200_LAYOUT_AOS) return fail(GEMB200_E_INVALID, "parameter draws need the row-per-env (AoS) I/O layout (per-env parameter blocks)");
+  const bool flux_limits = h->cfg.init_im_valid != 0;  // induction motor with random initial states: init_im is derived on the host
+  ParamDraw pd;
+  std::memset(&pd, 0, sizeof(pd));
+  bool seen[kMaxDraw] = {};
+  for (int j = 0; j < n; ++j) {
+    const int s = slot[j];
+    const bool motor = s >= 0 && s < GEMB200_MAX_MOTOR_PARAM, load = s >= GEMB200_MAX_MOTOR_PARAM && s <= GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_J_LOAD;
+    if (!motor && !load) return fail(GEMB200_E_INVALID, "unknown parameter slot (motor: GEMB200_MP_*, load: GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_A.._J_LOAD)");
+    if (s == GEMB200_MP_P) return fail(GEMB200_E_INVALID, "pole pairs cannot be drawn per env: the angle increments are prepared on the host per handle");
+    if (flux_limits && (s == GEMB200_MP_L_M || s == GEMB200_MP_L_SIGS || s == GEMB200_MP_L_SIGR || s == GEMB200_MP_R_S || s == GEMB200_MP_R_E))
+      return fail(GEMB200_E_INVALID, "l_m, l_sigs, l_sigr, r_s and r_r of an induction motor with random initial states enter the host-derived flux limits (init_im); not supported");
+    if (seen[s]) return fail(GEMB200_E_INVALID, "parameter slot given twice");
+    seen[s] = true;
+    if (kind[j] != GEMB200_DIST_UNIFORM && kind[j] != GEMB200_DIST_LOG_UNIFORM) return fail(GEMB200_E_INVALID, "unknown distribution kind");
+    if (!std::isfinite(lo[j]) || !std::isfinite(hi[j]) || lo[j] > hi[j]) return fail(GEMB200_E_INVALID, "distribution bounds must be finite with lo <= hi");
+    if (kind[j] == GEMB200_DIST_LOG_UNIFORM && !(lo[j] > 0)) return fail(GEMB200_E_INVALID, "log-uniform bounds must be positive");
+    pd.slot[j] = s; pd.kind[j] = kind[j]; pd.lo[j] = lo[j]; pd.hi[j] = hi[j];
+    if (kind[j] == GEMB200_DIST_LOG_UNIFORM) { pd.a[j] = std::log(lo[j]); pd.b[j] = std::log(hi[j]) - std::log(lo[j]); }
+    else { pd.a[j] = lo[j]; pd.b[j] = hi[j] - lo[j]; }
+  }
+  const size_t nn = (size_t)h->cfg.n_envs;
+  if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
+  if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, (size_t)kMaxDraw * nn * sizeof(double)));
+  if (!h->d_draw) CUDA_TRY(cudaMalloc(&h->d_draw, sizeof(ParamDraw)));
+  CUDA_TRY(cudaMemcpy(h->d_draw, &pd, sizeof(pd), cudaMemcpyHostToDevice));
+  if (!h->pf.envp) {  // no per-env blocks yet: every env starts from the shared parameters
+    RawParams raw;
+    for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
+    for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
+    const int grid = (int)((nn + 255) / 256);
+    if (h->cfg.dtype == GEMB200_F32) fill_env_params_kernel<float><<<grid, 256>>>(static_cast<float*>(h->d_envp), h->d_praw, h->pf.k, raw, (int)nn);
+    else fill_env_params_kernel<double><<<grid, 256>>>(static_cast<double*>(h->d_envp), h->d_praw, h->pd.k, raw, (int)nn);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaDeviceSynchronize());
+    h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
+    h->pf.plain = 0; h->pd.plain = 0;
+  }
+  h->n_draw = n;
+  h->pf.n_draw = n; h->pd.n_draw = n;
+  h->pf.draw = h->d_draw; h->pd.draw = h->d_draw;
+  h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
+  return GEMB200_OK;
+}
+
+int gemb200_get_env_params(gemb200_handle* h, void* out, void* stream) {
+  if (!h || !out) return fail(GEMB200_E_INVALID, "NULL argument");
+  if (h->n_draw == 0) return fail(GEMB200_E_INVALID, "no parameters are drawn (gemb200_set_param_randomization)");
+  DeviceGuard guard(h->cfg.device);
+  const int n = h->cfg.n_envs, grid = (n + 255) / 256;
+  if (h->cfg.dtype == GEMB200_F32) get_env_params_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(h->d_praw, h->d_draw, h->n_draw, static_cast<float*>(out), n);
+  else get_env_params_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>(h->d_praw, h->d_draw, h->n_draw, static_cast<double*>(out), n);
+  CUDA_TRY(cudaGetLastError());
   return GEMB200_OK;
 }
 
@@ -1248,6 +1298,7 @@ int64_t gemb200_checkpoint_size(gemb200_handle* h) {
 }
 int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob) {
   if (!h || !host_blob) return fail(GEMB200_E_INVALID, "NULL argument");
+  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
   DeviceGuard guard(h->cfg.device);
   CUDA_TRY(cudaDeviceSynchronize());
   if (h->dev_clock) { int rc = pull_clock(h, nullptr); if (rc) return rc; }  // the header carries the clock
@@ -1262,6 +1313,7 @@ int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob) {
 }
 int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob) {
   if (!h || !host_blob) return fail(GEMB200_E_INVALID, "NULL argument");
+  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
   DeviceGuard guard(h->cfg.device);
   CheckpointHeader want, got;
   make_header(h, &want);
@@ -1586,6 +1638,7 @@ int gemb200_query_env_record(const gemb200_config* cfg, int32_t* words, uint64_t
 
 int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
   if (m < 0) return fail(GEMB200_E_INVALID, "m must be >= 0");
   if (m == 0) return GEMB200_OK;
   if (!rows) return fail(GEMB200_E_INVALID, "rows is NULL");
@@ -1604,6 +1657,7 @@ int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint
 int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
                         const int32_t* env_idx, int32_t m, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
   if (m < 0 || n_rows < 0) return fail(GEMB200_E_INVALID, "m and n_rows must be >= 0");
   RecArgs a;
   record_args(h, &a);

@@ -56,15 +56,21 @@ enum : uint32_t {
   kStreamLaplace = 24, kStreamLaplaceR = 28,                  // Laplace walk increments (R: right after an in-kernel auto-reset)
   kStreamPeriodic = 32,                                       // + 2*slot (+1): sub-episode parameters of the periodic generators,
                                                               //   counter word 0 = step index of the sub-episode start
+  kStreamParam = 40, kStreamParamR = 48,                      // + j/4: parameter draws at a reset (reset_kernel; R: in-kernel auto-reset),
+                                                              //   one block of four uniforms per four drawn parameters
   kStreamNoise = 64,                                          // + 8*op + (state index >> 2): StateNoiseProcessor draws
   kStreamNoiseR = 128                                         //   ... right after an in-kernel auto-reset
 };
+
+// physical parameter slots of one env: GEMB200_MAX_MOTOR_PARAM motor slots, then 8 load slots (gemb200_set_param_randomization)
+constexpr int kMaxDraw = 16 + 8;
 
 // every stream id (base + its offsets) is used by exactly one consumer: ranges [base, base + width)
 constexpr bool streams_disjoint() {
   constexpr uint32_t r[][2] = {{kStreamWalk, 1}, {kStreamSubep, 1}, {kStreamInit, 1}, {kStreamWalkR, 1}, {kStreamSubepR, 1}, {kStreamInitState, 1}, {kStreamInitState2, 1},
                                {kStreamSupply, 1}, {kStreamSwitch, kMaxRef}, {kStreamSwitchR, kMaxRef}, {kStreamSubepHi, 1}, {kStreamSubepHiR, 1}, {kStreamLaplace, 1},
-                               {kStreamLaplaceR, 1}, {kStreamWalk2, 1}, {kStreamPeriodic, 2 * kMaxRef}, {kStreamNoise, 8 * kMaxStateOps}, {kStreamNoiseR, 8 * kMaxStateOps}};
+                               {kStreamLaplaceR, 1}, {kStreamWalk2, 1}, {kStreamPeriodic, 2 * kMaxRef}, {kStreamNoise, 8 * kMaxStateOps}, {kStreamNoiseR, 8 * kMaxStateOps},
+                               {kStreamParam, (kMaxDraw + 3) / 4}, {kStreamParamR, (kMaxDraw + 3) / 4}};
   constexpr int n = sizeof(r) / sizeof(r[0]);
   for (int a = 0; a < n; ++a)
     for (int b = a + 1; b < n; ++b)
@@ -84,6 +90,14 @@ struct Coef {
   real c[20];  // motor model coefficients
   real tq[4];  // torque coefficients
   real load_a, load_b, load_c, inv_j, omega_lim, omega_lin;
+};
+
+// Distributions of the parameters drawn at every reset (gemb200_set_param_randomization), in device memory behind StepParams::draw.
+// Draw j: v = a + b * U (uniform: a = lo, b = hi - lo; log-uniform: exp of it, a = log lo, b = log hi - log lo), clamped to [lo, hi].
+struct ParamDraw {
+  int32_t slot[kMaxDraw];  // parameter slot: GEMB200_MP_* or GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_*
+  int32_t kind[kMaxDraw];  // GEMB200_DIST_*
+  double a[kMaxDraw], b[kMaxDraw], lo[kMaxDraw], hi[kMaxDraw];
 };
 
 template <typename real>
@@ -237,6 +251,11 @@ struct StepParams {
   //      tensors; 0 destinations = the caller's tensors only ----
   int32_t n_dst;
   int64_t dst_delta[8];
+  // ---- parameter draws at every reset (gemb200_set_param_randomization; read by the ENVP instantiations and reset_kernel only).  Kept
+  //      at the end of the block so that the constant-bank offsets of every other field stay where they were ----
+  int32_t n_draw;          // parameters drawn per reset (0: none)
+  const ParamDraw* draw;   // their distributions
+  double* praw;            // [kMaxDraw][n] physical parameters of every env; drawn values are stored rounded to real
 };
 
 }  // namespace gemb200

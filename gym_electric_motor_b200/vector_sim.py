@@ -129,6 +129,40 @@ class VectorSim:
         lp = None if load_param is None else np.ascontiguousarray(load_param, dtype=np.float64).reshape(self.n, 8)
         vp = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)  # noqa: E731
         K.check(self._lib.gemb200_set_env_params(self._h, vp(mp), vp(lp)), "gemb200_set_env_params")
+        if mp is None and lp is None:
+            self._draw_slots = ()
+
+    _draw_slots = ()
+
+    @property
+    def randomized_slots(self):
+        """parameter slots drawn at every reset (gemb200_set_param_randomization), in the order of `env_params` rows"""
+        return self._draw_slots
+
+    def set_param_randomization(self, slots=(), kinds=(), lo=(), hi=()):
+        """Per-episode domain randomisation (gemb200_set_param_randomization): from now on every reset of an env draws new values for the
+        parameter slots (`_cabi.MP_*`, or `_cabi.MAX_MOTOR_PARAM + _cabi.LP_*`) from kinds[j] (`_cabi.DIST_*`) on [lo[j], hi[j]].  Draws
+        nothing by itself; empty arguments stop drawing (the envs keep their last values)."""
+        n = len(slots)
+        if not (len(kinds) == len(lo) == len(hi) == n):
+            raise ValueError("slots, kinds, lo and hi must have the same length")
+        m = max(n, 1)
+        K.check(self._lib.gemb200_set_param_randomization(self._h, n, (C.c_int32 * m)(*slots), (C.c_int32 * m)(*kinds),
+                                                         (C.c_double * m)(*lo), (C.c_double * m)(*hi)), "gemb200_set_param_randomization")
+        self._draw_slots = tuple(int(s) for s in slots)
+
+    def env_params(self):
+        """stored values of the drawn parameters, [len(randomized_slots), N] device tensor in the handle's dtype (stream-ordered copy)"""
+        if not self._draw_slots:
+            raise RuntimeError("no parameters are drawn per reset (set_param_randomization)")
+        out = torch.empty((len(self._draw_slots), self.n), dtype=self.dtype, device=self.device)
+        K.check(self._lib.gemb200_get_env_params(self._h, _ptr(out), self._stream()), "gemb200_get_env_params")
+        return out
+
+    def _refuse_while_drawing(self, what):
+        if self._draw_slots:
+            raise NotImplementedError(f"{what} is not available while parameters are drawn per reset: the drawn parameters are per-episode "
+                                      "state that neither checkpoints nor snapshot rows carry (DESIGN.md §7); stop the draws first")
 
     def step(self, action):
         """env.step: returns (obs, ref_next, reward, terminated) device tensors (views of reused buffers unless
@@ -226,12 +260,14 @@ class VectorSim:
         torch.cuda.current_stream(self.device).synchronize()
 
     def state_dict(self):
+        self._refuse_while_drawing("state_dict")
         size = self._lib.gemb200_checkpoint_size(self._h)
         buf = np.empty(size, dtype=np.uint8)
         K.check(self._lib.gemb200_checkpoint_save(self._h, buf.ctypes.data_as(C.c_void_p)), "gemb200_checkpoint_save")
         return {"blob": buf}
 
     def load_state_dict(self, sd):
+        self._refuse_while_drawing("load_state_dict")
         buf = np.ascontiguousarray(sd["blob"], dtype=np.uint8)
         if buf.size != self._lib.gemb200_checkpoint_size(self._h):
             raise ValueError("checkpoint size mismatch")
@@ -257,6 +293,7 @@ class VectorSim:
         Row j holds env idx[j]; a device index entry out of range leaves its row uninitialised."""
         from .snapshot import EnvSnapshot
 
+        self._refuse_while_drawing("snapshot")
         words, lid = self.record_layout()
         ii = self._dev_index(idx)
         m = self.n if ii is None else int(ii.numel())
@@ -270,6 +307,7 @@ class VectorSim:
         Device index entries out of range are skipped."""
         from .snapshot import check_layout
 
+        self._refuse_while_drawing("restore")
         words, lid = self.record_layout()
         check_layout(snap, words, lid)
         ii, rr = self._dev_index(idx), self._dev_index(rows)

@@ -348,6 +348,25 @@ int gemb200_get_clock(gemb200_handle* h, uint64_t* call_id, uint64_t* n_steps, v
  * Takes effect from the next reset / step; synchronises the device. */
 int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const double* load_param);
 
+/* Per-episode domain randomisation: from this call on, EVERY reset of an env (gemb200_reset, the in-kernel auto-reset of step and rollout,
+ * and therefore captured graphs) draws new values for n parameters from the env's own Philox stream, keyed by (seed, global env index,
+ * call id, stream), so equal seeds give equal parameter sequences independent of sharding.  slot[j]: GEMB200_MP_* for the motor,
+ * GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_* for the load; kind[j]: GEMB200_DIST_*; bounds lo[j] <= hi[j], finite, lo > 0 for log-uniform.
+ * A drawn value is rounded to the handle's dtype and stored; the env's coefficients are derived on the device from the stored values by
+ * the same code gemb200_set_env_params runs on the host, and the new episode (its reset observation included) uses them.  Parameters that
+ * are not drawn keep their per-env or shared value.  The call draws nothing itself: each env keeps its dynamics until its next reset.
+ * Without per-env blocks the call first fills them from the shared parameters, on the device.  n = 0: no more draws (the envs keep their
+ * last values); gemb200_set_env_params(h, NULL, NULL) returns to the shared coefficients and also ends the draws.
+ * Refused (GEMB200_E_INVALID): pole pairs (host-prepared angle increments), the flux-limit parameters l_m, l_sigs, l_sigr, r_s, r_r of an
+ * induction motor with random initial states (host-prepared init_im), the field-major (SoA) I/O layout, repeated or unknown slots and bad
+ * bounds.  While draws are on, gemb200_checkpoint_save / _load and gemb200_pack_envs / _unpack_envs return GEMB200_E_INVALID: the drawn
+ * parameters are per-episode state that neither format carries.  Synchronises the device. */
+enum gemb200_dist_kind { GEMB200_DIST_UNIFORM = 0, GEMB200_DIST_LOG_UNIFORM = 1 };
+int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t* slot, const int32_t* kind, const double* lo, const double* hi);
+/* Stream-ordered copy of the stored values of the drawn parameters into the device buffer out[n][n_envs] (handle dtype; order of the slots
+ * given to gemb200_set_param_randomization).  GEMB200_E_INVALID while no parameters are drawn. */
+int gemb200_get_env_params(gemb200_handle* h, void* out, void* stream);
+
 /* Fused aggregated return of the sharded layout (one process per GPU, SURVEY.md §8e: the ONE collective of the north star, done by the
  * step kernel itself instead of a separate NCCL all-gather).  Every rank owns a gather buffer (gemb200_peer_buffer_alloc: cudaMalloc +
  * IPC handle) of world sections; the ranks exchange the 64-byte handles out of band and map each other's buffers
