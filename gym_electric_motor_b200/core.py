@@ -355,34 +355,51 @@ class ElectricMotorEnvironment(_EnvBase):
         vals = sim.env_params()
         return {name: vals[j] for j, name in enumerate(self._randomized_names)}
 
-    def snapshot_envs(self, idx=None):
+    def snapshot_envs(self, idx=None, rng=False):
         """Branching support, the batched counterpart of `copy.deepcopy(env)`: the complete persistent state of envs `idx` (None: all;
         list, numpy array or tensor) as an `EnvSnapshot` of packed device rows, taken without a host synchronisation.  Host-side
-        indices are range-checked (IndexError); a device index tensor is taken as given.  Batched mode only."""
+        indices are range-checked (IndexError); a device index tensor is taken as given.  rng=True also takes the envs' RNG identities
+        (seed, global index and where their random streams stand), which `restore_envs(..., rng="source")` hands on.  Batched mode only."""
         if self._scalar:
             raise TypeError("snapshot_envs() needs a batched environment (num_envs=...)")
         from .snapshot import check_host_index
 
         sim = self._ensure_sim()
-        return sim.snapshot(check_host_index(idx, sim.n, "idx"))
+        idx = check_host_index(idx, sim.n, "idx")
+        return sim.snapshot(idx, rng=True) if rng else sim.snapshot(idx)
 
-    def restore_envs(self, snapshot, idx=None, rows=None):
+    def clear_rng_identities(self):
+        """Every env draws its own random numbers again (drops the identities adopted with `restore_envs(..., rng="source")`); afterwards
+        the envs draw exactly what they would have drawn had they never adopted one, and the env runs its shared-coefficient kernels again
+        unless it has per-env parameters of its own.  Batched mode only."""
+        if self._scalar:
+            raise TypeError("clear_rng_identities() needs a batched environment (num_envs=...)")
+        self._ensure_sim().clear_rng_ids()
+
+    def restore_envs(self, snapshot, idx=None, rows=None, rng="own"):
         """Env idx[j] (None: env j) takes the state of snapshot row rows[j] (None: row j): physically the source env, continuing bit for
-        bit except for the random numbers, which are the restored env's own from then on (its Wiener increments, periodic-generator
-        parameters, switching choices, noise and later random resets).  `rows` fans one snapshot out to many envs without copying it.
+        bit except for the random numbers, which by default (rng="own") are the restored env's own from then on (its Wiener increments,
+        periodic-generator parameters, switching choices, noise and later random resets).  `rows` fans one snapshot out to many envs without copying it.
         The snapshot may come from another env of the same kind and record layout (other num_envs or seed); another layout raises
         ValueError, host-side indices out of range IndexError.  Returns nothing: the observation rows of the restored envs are the
-        caller's to keep (the next step's outputs are computed from the restored state).  Batched mode only."""
+        caller's to keep (the next step's outputs are computed from the restored state).  Batched mode only.
+        rng="source" (a snapshot taken with rng=True) gives `copy.deepcopy(env)` semantics instead: every restored env adopts its source's
+        RNG identity and repeats the source's random numbers — same actions, same outputs, bit for bit, across terminations and resets.
+        A later restore with rng="own", `clear_rng_identities()` or `reset(seed=...)` drops the identity.  It needs the row-per-env layout
+        (ValueError); while identities are adopted, `state_dict` / `load_state_dict` raise NotImplementedError (DESIGN.md §7)."""
         if self._scalar:
             raise TypeError("restore_envs() needs a batched environment (num_envs=...)")
-        from .snapshot import check_host_index, check_layout
+        from .snapshot import check_host_index, check_layout, check_rng_mode
 
         sim = self._ensure_sim()
         words, lid = sim.record_layout()
         check_layout(snapshot, words, lid)
         idx = check_host_index(idx, sim.n, "idx")
         rows = check_host_index(rows, len(snapshot), "rows")
-        sim.restore(snapshot, idx, rows)
+        if check_rng_mode(snapshot, rng, sim.soa):
+            sim.restore(snapshot, idx, rows, rng="source")
+        else:
+            sim.restore(snapshot, idx, rows)
 
     def set_reference(self, values):
         """Push reference values [N, n_ref] for ExternalReferenceGenerator slots (used by the next step's reward)."""

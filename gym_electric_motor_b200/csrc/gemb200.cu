@@ -54,6 +54,8 @@ struct gemb200_handle {
   ParamDraw* d_draw = nullptr;  // distributions of the parameters drawn at every reset (gemb200_set_param_randomization)
   int n_draw = 0;               // parameters drawn per reset (0: none)
   void* d_imprev = nullptr;  // induction motors with random initial states [2][n]: initial currents of the env's previous episode
+  uint32_t* d_rngid = nullptr;  // RNG identities [kRngIdWords][n] (gemb200_adopt_rng_ids), allocated at the first adoption
+  bool ids_adopted = false;     // an identity was adopted since the last reseed / gemb200_clear_rng_ids
   int n_obs = 0, row_stride = 0;
   StepParams<float> pf;
   StepParams<double> pd;
@@ -878,7 +880,7 @@ int gemb200_destroy(gemb200_handle* h) {
   if (!h) return GEMB200_OK;
   DeviceGuard guard(h->cfg.device);
   cudaFree(h->d_st); cudaFree(h->d_stc); cudaFree(h->d_eps); cudaFree(h->d_sw); cudaFree(h->d_fifo); cudaFree(h->d_obsv); cudaFree(h->d_sup); cudaFree(h->d_supph); cudaFree(h->d_swst); cudaFree(h->d_ext); cudaFree(h->d_kenv); cudaFree(h->d_imprev); cudaFree(h->d_envp); cudaFree(h->d_clock);
-  cudaFree(h->d_praw); cudaFree(h->d_draw);
+  cudaFree(h->d_praw); cudaFree(h->d_draw); cudaFree(h->d_rngid);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_ref); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_mask);
   if (h->hstream) cudaStreamDestroy(h->hstream);
   for (int k = 0; k < 3; ++k) if (h->hpipe[k]) cudaStreamDestroy(h->hpipe[k]);
@@ -918,6 +920,7 @@ int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, voi
 // dicts): every env gets its own model coefficients, derived here exactly like the shared ones (the *_update_model methods,
 // mechanical_load.py:188-193) from ITS physical parameters.  Limits, nominal values, reward and reference settings stay those of the
 // handle's configuration.  NULL motor_param: back to the shared coefficients.
+static int fill_shared_blocks(gemb200_handle* h);
 int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const double* load_param) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   DeviceGuard guard(h->cfg.device);
@@ -925,8 +928,14 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   if (h->cfg.layout != GEMB200_LAYOUT_AOS && (motor_param || load_param))
     return fail(GEMB200_E_INVALID, "per-env parameter blocks need the row-per-env (AoS) I/O layout");
   if (!motor_param && !load_param) {
-    h->pf.envp = nullptr; h->pd.envp = nullptr;
     h->n_draw = 0; h->pf.n_draw = 0; h->pd.n_draw = 0;  // shared coefficients again: no parameter draws either
+    if (h->pf.rngid) {  // adopted RNG identities are read by the ENVP instantiations only: the blocks take the shared parameters instead
+      const int rc = fill_shared_blocks(h);
+      if (rc) return rc;
+      h->pf.coef_shared = h->pd.coef_shared = 1;
+      return GEMB200_OK;
+    }
+    h->pf.envp = nullptr; h->pd.envp = nullptr;
     h->pf.plain = h->pf.n_dst == 0 ? h->plain_shape : 0; h->pd.plain = h->pf.plain;
     return GEMB200_OK;
   }
@@ -963,6 +972,7 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
   h->pf.plain = 0; h->pd.plain = 0;  // the PLAIN instantiations read the shared constant-bank coefficients
   h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
+  h->pf.coef_shared = h->pd.coef_shared = 0;
   return GEMB200_OK;
 }
 
@@ -981,6 +991,35 @@ __global__ void fill_env_params_kernel(real* envp, double* praw, const Coef<real
   envp[24 * nn + i] = k.load_a; envp[25 * nn + i] = k.load_b; envp[26 * nn + i] = k.load_c;
   envp[27 * nn + i] = k.inv_j; envp[28 * nn + i] = k.omega_lim; envp[29 * nn + i] = k.omega_lin;
   for (int s = 0; s < kMaxDraw; ++s) praw[s * nn + i] = raw.v[s];
+}
+// no adopted identities any more: launches key every env by its own identity again, and blocks that only an adoption made go, so that the
+// handle runs its shared-coefficient kernels like a fresh one (the identity array stays allocated for the next adoption)
+static void drop_rng_ids(gemb200_handle* h) {
+  h->pf.rngid = h->pd.rngid = nullptr;
+  h->ids_adopted = false;
+  if (h->pf.coef_shared) {
+    h->pf.envp = nullptr; h->pd.envp = nullptr;
+    h->pf.plain = h->pf.n_dst == 0 ? h->plain_shape : 0; h->pd.plain = h->pf.plain;
+    h->pf.coef_shared = h->pd.coef_shared = 0;
+  }
+}
+// every env's block := the shared parameters (synchronises); the handle runs its ENVP instantiations from then on
+static int fill_shared_blocks(gemb200_handle* h) {
+  const size_t nn = (size_t)h->cfg.n_envs;
+  if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
+  if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, (size_t)kMaxDraw * nn * sizeof(double)));
+  RawParams raw;
+  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
+  for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
+  const int grid = (int)((nn + 255) / 256);
+  if (h->cfg.dtype == GEMB200_F32) fill_env_params_kernel<float><<<grid, 256>>>(static_cast<float*>(h->d_envp), h->d_praw, h->pf.k, raw, (int)nn);
+  else fill_env_params_kernel<double><<<grid, 256>>>(static_cast<double*>(h->d_envp), h->d_praw, h->pd.k, raw, (int)nn);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
+  h->pf.plain = 0; h->pd.plain = 0;
+  h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
+  return GEMB200_OK;
 }
 // out[j][i] = stored value of drawn parameter j of env i, in the handle's dtype
 template <typename real>
@@ -1023,23 +1062,13 @@ int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t*
     if (kind[j] == GEMB200_DIST_LOG_UNIFORM) { pd.a[j] = std::log(lo[j]); pd.b[j] = std::log(hi[j]) - std::log(lo[j]); }
     else { pd.a[j] = lo[j]; pd.b[j] = hi[j] - lo[j]; }
   }
-  const size_t nn = (size_t)h->cfg.n_envs;
-  if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
-  if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, (size_t)kMaxDraw * nn * sizeof(double)));
   if (!h->d_draw) CUDA_TRY(cudaMalloc(&h->d_draw, sizeof(ParamDraw)));
   CUDA_TRY(cudaMemcpy(h->d_draw, &pd, sizeof(pd), cudaMemcpyHostToDevice));
   if (!h->pf.envp) {  // no per-env blocks yet: every env starts from the shared parameters
-    RawParams raw;
-    for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
-    for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
-    const int grid = (int)((nn + 255) / 256);
-    if (h->cfg.dtype == GEMB200_F32) fill_env_params_kernel<float><<<grid, 256>>>(static_cast<float*>(h->d_envp), h->d_praw, h->pf.k, raw, (int)nn);
-    else fill_env_params_kernel<double><<<grid, 256>>>(static_cast<double*>(h->d_envp), h->d_praw, h->pd.k, raw, (int)nn);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaDeviceSynchronize());
-    h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
-    h->pf.plain = 0; h->pd.plain = 0;
+    const int rc = fill_shared_blocks(h);
+    if (rc) return rc;
   }
+  h->pf.coef_shared = h->pd.coef_shared = 0;  // the draws change the blocks: they are the caller's from now on
   h->n_draw = n;
   h->pf.n_draw = n; h->pd.n_draw = n;
   h->pf.draw = h->d_draw; h->pd.draw = h->d_draw;
@@ -1299,6 +1328,7 @@ int64_t gemb200_checkpoint_size(gemb200_handle* h) {
 int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob) {
   if (!h || !host_blob) return fail(GEMB200_E_INVALID, "NULL argument");
   if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  if (h->ids_adopted) return fail(GEMB200_E_INVALID, "checkpoints do not carry adopted RNG identities; clear them first (gemb200_clear_rng_ids, DESIGN §7)");
   DeviceGuard guard(h->cfg.device);
   CUDA_TRY(cudaDeviceSynchronize());
   if (h->dev_clock) { int rc = pull_clock(h, nullptr); if (rc) return rc; }  // the header carries the clock
@@ -1314,6 +1344,7 @@ int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob) {
 int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob) {
   if (!h || !host_blob) return fail(GEMB200_E_INVALID, "NULL argument");
   if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  if (h->ids_adopted) return fail(GEMB200_E_INVALID, "checkpoints do not carry adopted RNG identities; clear them first (gemb200_clear_rng_ids, DESIGN §7)");
   DeviceGuard guard(h->cfg.device);
   CheckpointHeader want, got;
   make_header(h, &want);
@@ -1350,6 +1381,7 @@ int gemb200_reseed(gemb200_handle* h, uint64_t seed, void* stream) {
     h->pf.rk[r][0] = lo; h->pf.rk[r][1] = hi; h->pd.rk[r][0] = lo; h->pd.rk[r][1] = hi;
   }
   h->pf.seed_lo = h->pd.seed_lo = (uint32_t)seed; h->pf.seed_hi = h->pd.seed_hi = (uint32_t)(seed >> 32);
+  drop_rng_ids(h);  // every env draws with its own identity again
   Section s[16];
   const int k = sections(h, s);
   for (int i = 0; i < k; ++i) {
@@ -1421,9 +1453,18 @@ struct RecArgs {
   uint32_t kstep;                // step count (sub-episode clock) and dead-time ring position of the host clock ...
   int32_t ring;
   const uint32_t* clock_dev;     // ... or of the device-resident clock (gemb200_set_device_clock), read like clock_of() does
+  uint32_t* rngid;               // RNG identities [kRngIdWords][n] (nullptr: none adopted yet); unpack gives the envs their own back
+  uint32_t seed_lo, seed_hi;
+  int64_t env_offset;
 };
 constexpr int kRecBlockMax = 128;
 
+// env i's own RNG identity: the handle's seed, its global index, no offsets (the keying of an env that adopted none)
+__device__ __forceinline__ void set_own_rng_id(uint32_t* ids, size_t n, unsigned i, uint32_t seed_lo, uint32_t seed_hi, int64_t env_offset) {
+  const uint64_t g = (uint64_t)(env_offset + i);
+  ids[i] = seed_lo; ids[n + i] = seed_hi; ids[2 * n + i] = (uint32_t)g; ids[3 * n + i] = (uint32_t)(g >> 32);
+  ids[4 * n + i] = 0u; ids[5 * n + i] = 0u; ids[6 * n + i] = 0u; ids[7 * n + i] = 0u;
+}
 __device__ __forceinline__ void rec_clock(const RecArgs& a, uint32_t* kstep, int* ring) {
   if (a.clock_dev) { *kstep = a.clock_dev[2]; *ring = (int)a.clock_dev[3]; }
   else { *kstep = a.kstep; *ring = a.ring; }
@@ -1563,6 +1604,7 @@ __global__ void __launch_bounds__(kRecBlockMax) unpack_envs_kernel(const RecArgs
     uint32_t* row = srow + t * a.stride;
     rebase_row(a, row, kstep);
     move_env<false>(a, (unsigned)i, ring, row);
+    if (a.rngid) set_own_rng_id(a.rngid, (size_t)a.n, (unsigned)i, a.seed_lo, a.seed_hi, a.env_offset);
   }
 }
 
@@ -1618,6 +1660,9 @@ static void record_args(gemb200_handle* h, RecArgs* a) {
   a->kstep = (uint32_t)h->n_steps;
   a->ring = a->dead > 0 ? (int)(h->n_steps % (uint64_t)a->dead) : 0;
   a->clock_dev = h->dev_clock ? h->d_clock : nullptr;
+  a->rngid = h->pf.rngid ? h->d_rngid : nullptr;
+  a->seed_lo = (uint32_t)h->cfg.seed; a->seed_hi = (uint32_t)(h->cfg.seed >> 32);
+  a->env_offset = h->cfg.env_index_offset;
 }
 static int record_block(int stride) {  // largest block whose rows fit the default 48 KB of shared memory
   for (int b = kRecBlockMax; b >= 32; b >>= 1)
@@ -1672,6 +1717,122 @@ int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows,
   unpack_envs_kernel<<<grid, block, (size_t)block * a.stride * sizeof(uint32_t), (cudaStream_t)stream>>>(a, rows, n_rows, row_idx, env_idx, m);
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
+  return GEMB200_OK;
+}
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------------------------
+// RNG identities (gemb200_pack_rng_ids / gemb200_adopt_rng_ids / gemb200_clear_rng_ids; row format in include/gemb200.h)
+// ----------------------------------------------------------------------------------------------------------------
+static_assert(kRngIdWords == GEMB200_RNG_ID_WORDS, "RNG identity row width");
+// the handle's clock as the identities see it: the call id of the NEXT call and the step count, from the host counters or d_clock
+struct IdClockArgs { uint64_t call; uint32_t steps; const uint32_t* dev; };
+__device__ __forceinline__ void id_clock_now(const IdClockArgs& c, uint64_t* call, uint32_t* steps) {
+  if (c.dev) { *call = ((uint64_t)c.dev[1] << 32) | c.dev[0]; *steps = c.dev[2]; }
+  else { *call = c.call; *steps = c.steps; }
+}
+static IdClockArgs id_clock_args(const gemb200_handle* h) { return IdClockArgs{h->gstep + 1, (uint32_t)h->n_steps, h->dev_clock ? h->d_clock : nullptr}; }
+
+__global__ void own_rng_ids_kernel(uint32_t* ids, int n, uint32_t seed_lo, uint32_t seed_hi, int64_t env_offset) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) set_own_rng_id(ids, (size_t)n, (unsigned)i, seed_lo, seed_hi, env_offset);
+}
+// one thread per output word: row j of env env_idx[j] = its effective identity (ids NULL: every env has its own), the rows written contiguously
+__global__ void pack_rng_ids_kernel(const uint32_t* __restrict__ ids, int n, uint32_t seed_lo, uint32_t seed_hi, int64_t env_offset, const IdClockArgs c,
+                                    const int32_t* __restrict__ env_idx, int m, uint32_t* __restrict__ out) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= (int64_t)m * kRngIdWords) return;
+  const int j = (int)(k / kRngIdWords), w = (int)(k % kRngIdWords);
+  const int i = env_idx ? env_idx[j] : j;
+  if (i < 0 || i >= n) return;
+  const size_t nn = (size_t)n;
+  const uint64_t g = (uint64_t)(env_offset + i);
+  uint64_t call;
+  uint32_t steps, v = 0u;
+  id_clock_now(c, &call, &steps);
+  if (w < 4) v = ids ? ids[w * nn + i] : (w == 0 ? seed_lo : (w == 1 ? seed_hi : (w == 2 ? (uint32_t)g : (uint32_t)(g >> 32))));
+  else if (w < 6) {
+    const uint64_t e = call + (ids ? (((uint64_t)ids[5 * nn + i] << 32) | ids[4 * nn + i]) : 0u);
+    v = w == 4 ? (uint32_t)e : (uint32_t)(e >> 32);
+  } else if (w == 6) v = steps + (ids ? ids[6 * nn + i] : 0u);
+  out[k] = v;
+}
+// env env_idx[j] takes identity row row_idx[j]: its key and global index, and offsets that map this handle's clock onto the source's
+__global__ void adopt_rng_ids_kernel(uint32_t* __restrict__ ids, int n, const IdClockArgs c, const uint32_t* __restrict__ rows, int n_rows,
+                                     const int32_t* __restrict__ row_idx, const int32_t* __restrict__ env_idx, int m) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= m) return;
+  const int r = row_idx ? row_idx[j] : j, i = env_idx ? env_idx[j] : j;
+  if (r < 0 || r >= n_rows || i < 0 || i >= n) return;
+  uint32_t w[kRngIdWords];
+#pragma unroll
+  for (int q = 0; q < kRngIdWords; ++q) w[q] = __ldg(rows + (size_t)r * kRngIdWords + q);
+  uint64_t call;
+  uint32_t steps;
+  id_clock_now(c, &call, &steps);
+  const uint64_t dcall = (((uint64_t)w[5] << 32) | w[4]) - call;
+  const size_t nn = (size_t)n;
+  ids[i] = w[0]; ids[nn + i] = w[1]; ids[2 * nn + i] = w[2]; ids[3 * nn + i] = w[3];
+  ids[4 * nn + i] = (uint32_t)dcall; ids[5 * nn + i] = (uint32_t)(dcall >> 32); ids[6 * nn + i] = w[6] - steps; ids[7 * nn + i] = 0u;
+}
+
+static int launch_own_rng_ids(gemb200_handle* h, cudaStream_t st) {
+  const int n = h->cfg.n_envs;
+  own_rng_ids_kernel<<<(n + 255) / 256, 256, 0, st>>>(h->d_rngid, n, (uint32_t)h->cfg.seed, (uint32_t)(h->cfg.seed >> 32), h->cfg.env_index_offset);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return GEMB200_OK;
+}
+
+extern "C" {
+
+int gemb200_pack_rng_ids(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* ids, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (m < 0) return fail(GEMB200_E_INVALID, "m must be >= 0");
+  if (m == 0) return GEMB200_OK;
+  if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
+  DeviceGuard guard(h->cfg.device);
+  const int64_t words = (int64_t)m * kRngIdWords;
+  pack_rng_ids_kernel<<<(unsigned)((words + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->pf.rngid ? h->d_rngid : nullptr, h->cfg.n_envs, (uint32_t)h->cfg.seed,
+                                                                                        (uint32_t)(h->cfg.seed >> 32), h->cfg.env_index_offset, id_clock_args(h), env_idx, m, ids);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return GEMB200_OK;
+}
+
+int gemb200_adopt_rng_ids(gemb200_handle* h, const uint32_t* ids, int32_t n_ids, const int32_t* row_idx, const int32_t* env_idx, int32_t m, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (h->cfg.layout != GEMB200_LAYOUT_AOS)
+    return fail(GEMB200_E_INVALID, "adopted RNG identities are read by the per-env parameter instantiations, which need the row-per-env (AoS) I/O layout (DESIGN §7)");
+  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "RNG identities cannot be adopted while parameters are drawn per reset: snapshots are refused then (DESIGN §7)");
+  if (m < 0 || n_ids < 0) return fail(GEMB200_E_INVALID, "m and n_ids must be >= 0");
+  if (m == 0 || n_ids == 0) return GEMB200_OK;
+  if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
+  DeviceGuard guard(h->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!h->pf.envp) {  // first adoption: the shared parameters into per-env blocks, so that the handle runs the ENVP instantiations (synchronises)
+    const int rc = fill_shared_blocks(h);
+    if (rc) return rc;
+    h->pf.coef_shared = h->pd.coef_shared = 1;
+  }
+  if (!h->d_rngid) CUDA_TRY(cudaMalloc(&h->d_rngid, (size_t)kRngIdWords * (size_t)h->cfg.n_envs * sizeof(uint32_t)));
+  if (!h->pf.rngid) {  // every other env keeps its own identity
+    const int rc = launch_own_rng_ids(h, st);
+    if (rc) return rc;
+    h->pf.rngid = h->pd.rngid = h->d_rngid;
+  }
+  adopt_rng_ids_kernel<<<(m + 255) / 256, 256, 0, st>>>(h->d_rngid, h->cfg.n_envs, id_clock_args(h), ids, n_ids, row_idx, env_idx, m);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  h->ids_adopted = true;
+  return GEMB200_OK;
+}
+
+int gemb200_clear_rng_ids(gemb200_handle* h, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  (void)stream;  // launches enqueued before the call keep the identities they were launched with
+  drop_rng_ids(h);
   return GEMB200_OK;
 }
 

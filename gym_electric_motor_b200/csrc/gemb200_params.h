@@ -256,6 +256,12 @@ struct StepParams {
   int32_t n_draw;          // parameters drawn per reset (0: none)
   const ParamDraw* draw;   // their distributions
   double* praw;            // [kMaxDraw][n] physical parameters of every env; drawn values are stored rounded to real
+  // ---- adopted RNG identities (gemb200_adopt_rng_ids; read by the ENVP instantiations and reset_kernel only, once per launch):
+  //      [kRngIdWords][n] u32 = Philox key lo, hi | global env index lo, hi | call-id offset lo, hi | step offset | spare.
+  //      nullptr: every env draws with its own identity (seed, env_offset + i, 0, 0) ----
+  const uint32_t* rngid;
+  int32_t coef_shared;     // 1: the per-env blocks hold the shared parameters (made by the first adoption): reset observations from reset_obs
 };
+constexpr int kRngIdWords = 8;
 
 }  // namespace gemb200

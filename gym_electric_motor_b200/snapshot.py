@@ -4,24 +4,31 @@ An `EnvSnapshot` holds the complete persistent state of m envs as packed rows (g
 plain device `torch.int32` tensor [m, words] that the caller may keep, concatenate, index or send to another rank, and that
 `VectorSim.restore` / `ElectricMotorEnvironment.restore_envs` put into any envs of a handle with the same record layout — the same env in
 another batch size, seed or index offset, or with other per-env parameters.  A restored env continues exactly like its source, except
-that it draws the random numbers of its own (seed, global env index) from then on.
+that it draws the random numbers of its own (seed, global env index) from then on — unless the snapshot was taken with `rng=True` and is
+restored with `rng="source"`: the env then adopts its source's RNG identity and repeats the source's draws (copy.deepcopy semantics).
 """
 import numpy as np
 import torch
 
+from ._cabi import RNG_ID_WORDS
+
 
 class EnvSnapshot:
-    """Packed state of m envs: `rows` [m, words] int32 on the device, `layout_id` of the record layout, `dtype` of the handle's state.
+    """Packed state of m envs: `rows` [m, words] int32 on the device, `layout_id` of the record layout, `dtype` of the handle's state,
+    `rng` [m, RNG_ID_WORDS] int32 = the envs' RNG identities (gemb200_pack_rng_ids) or None.
     `len(snap)` is m; `snap[k]`, `snap[a:b]`, `snap[index list / tensor]` are sub-snapshots of the selected rows."""
 
-    __slots__ = ("rows", "layout_id", "dtype")
+    __slots__ = ("rows", "layout_id", "dtype", "rng")
 
-    def __init__(self, rows, layout_id, dtype):
+    def __init__(self, rows, layout_id, dtype, rng=None):
         if not isinstance(rows, torch.Tensor) or rows.dtype != torch.int32 or rows.dim() != 2:
             raise ValueError("EnvSnapshot rows must be a 2-D torch.int32 tensor [m, words]")
+        if rng is not None and (not isinstance(rng, torch.Tensor) or rng.dtype != torch.int32 or tuple(rng.shape) != (rows.shape[0], RNG_ID_WORDS)):
+            raise ValueError(f"EnvSnapshot rng must be a torch.int32 tensor [m, {RNG_ID_WORDS}] with one row per snapshot row")
         self.rows = rows
         self.layout_id = int(layout_id)
         self.dtype = dtype
+        self.rng = rng
 
     def __len__(self):
         return int(self.rows.shape[0])
@@ -35,15 +42,17 @@ class EnvSnapshot:
             k = int(idx) + (len(self) if int(idx) < 0 else 0)
             if not 0 <= k < len(self):
                 raise IndexError(f"snapshot index {idx} out of range for {len(self)} rows")
-            sub = self.rows[k:k + 1]
+            sel = slice(k, k + 1)
         elif isinstance(idx, slice):
-            sub = self.rows[idx]
+            sel = idx
         else:
-            sub = self.rows[torch.as_tensor(np.asarray(idx) if not isinstance(idx, torch.Tensor) else idx, device=self.rows.device).long()]
-        return EnvSnapshot(sub.contiguous(), self.layout_id, self.dtype)
+            sel = torch.as_tensor(np.asarray(idx) if not isinstance(idx, torch.Tensor) else idx, device=self.rows.device).long()
+        rng = None if self.rng is None else self.rng[sel if isinstance(sel, slice) else sel.to(self.rng.device)].contiguous()
+        return EnvSnapshot(self.rows[sel].contiguous(), self.layout_id, self.dtype, rng)
 
     def __repr__(self):
-        return f"EnvSnapshot(m={len(self)}, words={self.words}, layout_id={self.layout_id:#018x}, dtype={self.dtype})"
+        return (f"EnvSnapshot(m={len(self)}, words={self.words}, layout_id={self.layout_id:#018x}, dtype={self.dtype}, "
+                f"rng={'yes' if self.rng is not None else 'no'})")
 
 
 def check_host_index(idx, bound, what):
@@ -57,6 +66,19 @@ def check_host_index(idx, bound, what):
     if a.size and (a.min() < 0 or a.max() >= bound):
         raise IndexError(f"{what} out of range: entries must be in [0, {bound})")
     return a
+
+
+def check_rng_mode(snap, rng, soa):
+    """the `rng` argument of a restore: "own" (the envs keep drawing their own numbers) or "source" (they adopt the snapshot's RNG
+    identities, which need a snapshot taken with rng=True and the row-per-env layout); ValueError otherwise"""
+    if rng not in ("own", "source"):
+        raise ValueError(f"rng must be 'own' or 'source', got {rng!r}")
+    if rng == "source":
+        if snap.rng is None:
+            raise ValueError("rng='source' needs a snapshot taken with rng=True (it carries no RNG identities)")
+        if soa:
+            raise ValueError("adopted RNG identities need the row-per-env layout (layout='aos'), like per-env parameter blocks (DESIGN.md §7)")
+    return rng == "source"
 
 
 def check_layout(snap, words, layout_id):

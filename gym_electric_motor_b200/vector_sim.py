@@ -109,6 +109,7 @@ class VectorSim:
         """re-key the RNG streams and start the handle over (gemb200_reseed): equal seeds -> identical episodes"""
         K.check(self._lib.gemb200_reseed(self._h, C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), self._stream()), "gemb200_reseed")
         self.cfg.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._ids_adopted = False  # the reseed gives every env its own RNG identity back
 
     def set_device_clock(self, enable=True):
         """Device-resident clock (gemb200_set_device_clock): while on, step / rollout / reset launches read the RNG call id, the step count
@@ -158,6 +159,13 @@ class VectorSim:
         out = torch.empty((len(self._draw_slots), self.n), dtype=self.dtype, device=self.device)
         K.check(self._lib.gemb200_get_env_params(self._h, _ptr(out), self._stream()), "gemb200_get_env_params")
         return out
+
+    _ids_adopted = False
+
+    def _refuse_with_identities(self, what):
+        if self._ids_adopted:
+            raise NotImplementedError(f"{what} is not available while envs hold adopted RNG identities (restore(..., rng='source')): the "
+                                      "checkpoint does not carry them (DESIGN.md §7); clear_rng_ids() or reseed first")
 
     def _refuse_while_drawing(self, what):
         if self._draw_slots:
@@ -261,6 +269,7 @@ class VectorSim:
 
     def state_dict(self):
         self._refuse_while_drawing("state_dict")
+        self._refuse_with_identities("state_dict")
         size = self._lib.gemb200_checkpoint_size(self._h)
         buf = np.empty(size, dtype=np.uint8)
         K.check(self._lib.gemb200_checkpoint_save(self._h, buf.ctypes.data_as(C.c_void_p)), "gemb200_checkpoint_save")
@@ -268,6 +277,7 @@ class VectorSim:
 
     def load_state_dict(self, sd):
         self._refuse_while_drawing("load_state_dict")
+        self._refuse_with_identities("load_state_dict")
         buf = np.ascontiguousarray(sd["blob"], dtype=np.uint8)
         if buf.size != self._lib.gemb200_checkpoint_size(self._h):
             raise ValueError("checkpoint size mismatch")
@@ -288,9 +298,10 @@ class VectorSim:
         t = idx if isinstance(idx, torch.Tensor) else torch.as_tensor(np.asarray(idx, dtype=np.int64).reshape(-1))
         return t.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
 
-    def snapshot(self, idx=None):
+    def snapshot(self, idx=None, rng=False):
         """Pack the persistent state of envs `idx` (None: all) into an EnvSnapshot (gemb200_pack_envs; stream-ordered, no host sync).
-        Row j holds env idx[j]; a device index entry out of range leaves its row uninitialised."""
+        Row j holds env idx[j]; a device index entry out of range leaves its row uninitialised.  rng=True also packs the envs' effective
+        RNG identities (gemb200_pack_rng_ids) into `snap.rng`, for restore(..., rng="source")."""
         from .snapshot import EnvSnapshot
 
         self._refuse_while_drawing("snapshot")
@@ -299,26 +310,41 @@ class VectorSim:
         m = self.n if ii is None else int(ii.numel())
         rows = torch.empty((m, words), dtype=torch.int32, device=self.device)
         K.check(self._lib.gemb200_pack_envs(self._h, _ptr(ii), m, _ptr(rows), self._stream()), "gemb200_pack_envs")
-        return EnvSnapshot(rows, lid, self.dtype)
+        ids = None
+        if rng:
+            ids = torch.empty((m, K.RNG_ID_WORDS), dtype=torch.int32, device=self.device)
+            K.check(self._lib.gemb200_pack_rng_ids(self._h, _ptr(ii), m, _ptr(ids), self._stream()), "gemb200_pack_rng_ids")
+        return EnvSnapshot(rows, lid, self.dtype, ids)
 
-    def restore(self, snap, idx=None, rows=None):
+    def clear_rng_ids(self):
+        """every env draws with its own RNG identity again (gemb200_clear_rng_ids; stream-ordered)"""
+        K.check(self._lib.gemb200_clear_rng_ids(self._h, self._stream()), "gemb200_clear_rng_ids")
+        self._ids_adopted = False
+
+    def restore(self, snap, idx=None, rows=None, rng="own"):
         """Env idx[j] (None: j) takes the state of snapshot row rows[j] (None: j) (gemb200_unpack_envs; stream-ordered, no host sync).
         `rows` fans one snapshot out: restore(snap, idx=range(C * m), rows=np.repeat(range(m), C)) copies every row into C envs.
-        Device index entries out of range are skipped."""
-        from .snapshot import check_layout
+        Device index entries out of range are skipped.  rng="own": the envs draw their own random numbers from then on; rng="source": they
+        adopt the snapshot's RNG identities (gemb200_adopt_rng_ids) and repeat their sources' draws."""
+        from .snapshot import check_layout, check_rng_mode
 
         self._refuse_while_drawing("restore")
         words, lid = self.record_layout()
         check_layout(snap, words, lid)
+        adopt = check_rng_mode(snap, rng, self.soa)
         ii, rr = self._dev_index(idx), self._dev_index(rows)
         if ii is not None and rr is not None and ii.numel() != rr.numel():
             raise ValueError(f"idx ({ii.numel()}) and rows ({rr.numel()}) must have the same length")
         m = int(ii.numel()) if ii is not None else (int(rr.numel()) if rr is not None else min(len(snap), self.n))
-        if snap.rows.device != self.device:
+        if snap.rows.device != self.device or (adopt and snap.rng.device != self.device):
             raise ValueError(f"snapshot rows are on {snap.rows.device}, this handle on {self.device}: move the rows first")
         data = snap.rows.contiguous()
         K.check(self._lib.gemb200_unpack_envs(self._h, _ptr(data), len(snap), C.c_uint64(lid), _ptr(rr), _ptr(ii), m, self._stream()),
                 "gemb200_unpack_envs")
+        if adopt:
+            ids = snap.rng.contiguous()
+            K.check(self._lib.gemb200_adopt_rng_ids(self._h, _ptr(ids), len(snap), _ptr(rr), _ptr(ii), m, self._stream()), "gemb200_adopt_rng_ids")
+            self._ids_adopted = True
 
     # ------------------------------------------------------------------ measurement helpers
     @property

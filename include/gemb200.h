@@ -417,7 +417,7 @@ int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob);
  * bit pattern in fp32, the integral double value in fp64): the sub-episode ends, the start step of a slot whose current generator is
  * periodic (sinus / step / sawtooth / triangular), and the super-episode ends.  Unpack re-bases them on the destination's step count.
  * Not in the row: the per-env parameter table (configuration, like in the checkpoint) and the RNG identity — a restored env draws the
- * random numbers of ITS OWN (seed, global index) from then on.
+ * random numbers of ITS OWN (seed, global index) from then on, unless it adopts its source's (gemb200_adopt_rng_ids below).
  * layout_id: FNV-1a over what decides the row format (dtype, motor, n_ode, n_ref, generator kinds and switched grouping, switching-state
  * array, dead time and its order and queue width, state-op kinds, supply, external speed load, induction motor with random initial
  * states); not over n_envs, seed, offsets, device, tau, solver, parameters, limits, reward, constraints, autoreset or layout. */
@@ -429,6 +429,35 @@ int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint
  * of another layout_id with GEMB200_E_INVALID */
 int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
                         const int32_t* env_idx, int32_t m, void* stream);
+
+/* RNG identities: copy.deepcopy(env) semantics for restored envs (opt-in; DESIGN §7).  Every random draw of an env is keyed by its
+ * identity: a Philox key, a global env index, an RNG call-id offset and a step offset — by default the handle's seed, env_index_offset + i,
+ * 0 and 0.  gemb200_pack_rng_ids exports the EFFECTIVE identity of chosen envs as rows of GEMB200_RNG_ID_WORDS uint32:
+ *   [0] key lo  [1] key hi  [2] global env index lo  [3] hi  [4] call id of the env's next call lo  [5] hi  [6] its step count  [7] 0
+ * (taken from the handle's clock; with the device clock on, from device memory).  gemb200_adopt_rng_ids gives env env_idx[j] (NULL: j)
+ * identity row row_idx[j] (NULL: j): it stores the row's key and index and the differences between the row's call id / step count and
+ * this handle's at the time of the call.  From then on every draw of that env — step, rollout, reset (masked or not), in-kernel auto-reset
+ * and captured graphs; reference walks, sub-episodes, periodic and switched generators, initial values, random initial states, supply
+ * phase, state noise, parameter draws — uses that identity.  Replay property: pack env s of handle A with gemb200_pack_envs and
+ * gemb200_pack_rng_ids, unpack and adopt both into env d of handle B (other n_envs, seed or env_index_offset allowed, the same handle
+ * too); the same sequence of calls on A and B with the same actions for s and d then gives env d bit for bit the outputs of env s.
+ * Packing an env that holds an adopted identity exports it advanced to now, so a branch of a branch replays the original.
+ * gemb200_unpack_envs gives the destination envs their own identity back; gemb200_reseed and gemb200_clear_rng_ids give it back to every
+ * env and return a handle whose per-env parameter blocks only the adoption made to its shared-coefficient kernels.  Adoption needs the row-per-env I/O layout and is refused while parameters are drawn per reset (GEMB200_E_INVALID); while an
+ * identity is adopted (until gemb200_clear_rng_ids or gemb200_reseed) gemb200_checkpoint_save / _load return GEMB200_E_INVALID: the blob
+ * carries no identities.  The first adoption on a handle without per-env parameter blocks fills them from the shared parameters
+ * (synchronises the device, not capturable); from then on the handle runs its per-env parameter kernels.  All calls are stream-ordered,
+ * take device pointers and skip out-of-range entries; apart from that first adoption they never synchronise and can be captured.
+ * A CUDA graph keeps the launch parameters it was captured with: capture step / rollout / reset launches AFTER the first adoption (and
+ * again after gemb200_clear_rng_ids or gemb200_reseed) for them to read the identities; adoptions into a handle whose identities are in use
+ * are seen by graphs captured since then. */
+#define GEMB200_RNG_ID_WORDS 8
+/* ids[j][0..GEMB200_RNG_ID_WORDS) = effective identity of env env_idx[j] (env_idx NULL: env j), j < m */
+int gemb200_pack_rng_ids(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* ids, void* stream);
+/* env env_idx[j] (NULL: j) adopts identity row ids[row_idx[j]] (NULL: row j), j < m; row_idx entries index [0, n_ids) */
+int gemb200_adopt_rng_ids(gemb200_handle* h, const uint32_t* ids, int32_t n_ids, const int32_t* row_idx, const int32_t* env_idx, int32_t m, void* stream);
+/* every env draws with its own identity again */
+int gemb200_clear_rng_ids(gemb200_handle* h, void* stream);
 
 /* Introspection used by bench.py: number of kernel launches issued through this handle so far, and the
  * CUDA-event time in ms of the step launches since the last call (see DESIGN.md "Measurement"). */

@@ -1,6 +1,6 @@
 """Per-env snapshot throughput (gemb200_pack_envs / gemb200_unpack_envs) and a random-shooting MPC control step built on it.
 
-    python tools/branch_bench.py [--envs 1048576] [--reps 20]
+    python tools/branch_bench.py [--envs 1048576] [--reps 20] [--rng own|source]
 
 Prints the GPU name and power limit, then one JSON line per measurement (CUDA events, median over --reps):
   1. pack and unpack of all envs of Cont-CC-PMSM-v0 (fp32: 11 words = 44 B per env), bytes moved and the fraction of the H100 SXM data-sheet
@@ -9,6 +9,11 @@ Prints the GPU name and power limit, then one JSON line per measurement (CUDA ev
   3. a random-shooting MPC control step, 1024 plants x 1024 candidates x horizon 8: pack the plants, fan them out into the model handle,
      rollout recording only the rewards, sum over the horizon, argmax per plant, step the plants with the first action of their best
      branch.  The candidate actions are drawn once up front (their generation is the policy's cost, not the simulator's).
+--rng source (copy.deepcopy semantics: every candidate adopts its plant's RNG identity, so all candidates of a plant are scored against
+the same future reference) packs the identities with the rows and adopts them with the fan-out, in 1.-3. alike.  Before timing it checks
+that the candidates of every plant record identical reference trajectories until they terminate.  It then prints a fourth line:
+  4. microseconds per env step of a fused rollout of --envs envs recording every step for 32 steps, auto-reset on, in three arms taking
+     turns: shared coefficients, per-env parameter blocks that hold the shared parameters, and the same blocks with adopted identities.
 Run from the repository root after the build; writes nothing.
 """
 import argparse
@@ -17,6 +22,7 @@ import os
 import subprocess
 import sys
 
+import numpy as np
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
@@ -63,7 +69,11 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--plants", type=int, default=1024)
     ap.add_argument("--horizon", type=int, default=8)
+    ap.add_argument("--rng", choices=("own", "source"), default="own")
     args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: this benchmark measures the GPU and has no CPU fallback")
+    ids = args.rng == "source"
     name, plimit = gpu_info()
     print(f"GPU: {name}, power limit {plimit}")
     n = args.envs
@@ -71,23 +81,27 @@ def main():
     sim.reset()
     words, _ = sim.record_layout()
     rec_bytes = 4 * words
-    snap = sim.snapshot()
+    mode = "source" if ids else "own"
+    id_bytes = 4 * 8 if ids else 0  # GEMB200_RNG_ID_WORDS words per env: identity array and identity rows
+    snap = sim.snapshot(rng=ids)
     torch.cuda.synchronize()
 
-    ms = timed(lambda: sim.snapshot(), args.reps)
-    moved = 2 * rec_bytes * n  # state read + rows written
-    print(json.dumps(dict(what="pack", envs=n, words=words, ms=round(ms, 4), bytes=moved, tb_s=round(moved / ms / 1e9, 3),
+    ms = timed(lambda: sim.snapshot(rng=ids), args.reps)
+    moved = 2 * (rec_bytes + id_bytes) * n  # state (and identities) read + rows written
+    print(json.dumps(dict(what="pack", rng=mode, envs=n, words=words, ms=round(ms, 4), bytes=moved, tb_s=round(moved / ms / 1e9, 3),
                           frac_datasheet=round(moved / ms / 1e-3 / PEAK, 3))))
-    ms = timed(lambda: sim.restore(snap), args.reps)
-    print(json.dumps(dict(what="unpack", envs=n, words=words, ms=round(ms, 4), bytes=moved, tb_s=round(moved / ms / 1e9, 3),
+    ms = timed(lambda: sim.restore(snap, rng=mode), args.reps)
+    print(json.dumps(dict(what="unpack", rng=mode, envs=n, words=words, ms=round(ms, 4), bytes=moved, tb_s=round(moved / ms / 1e9, 3),
                           frac_datasheet=round(moved / ms / 1e-3 / PEAK, 3))))
 
     m = 1024
     few = snap[:m]
     ridx = torch.arange(m, device=sim.device, dtype=torch.int32).repeat_interleave(n // m)
-    ms = timed(lambda: sim.restore(few, rows=ridx), args.reps)
-    moved_f = (rec_bytes + 4) * n + rec_bytes * m  # state written + row index read + the (L2-resident) rows once
-    print(json.dumps(dict(what="fan_out_unpack", rows=m, envs=n, ms=round(ms, 4), bytes=moved_f, tb_s=round(moved_f / ms / 1e9, 3),
+    ms = timed(lambda: sim.restore(few, rows=ridx, rng=mode), args.reps)
+    # state written + row index read + the (L2-resident) rows once; with identities the own identity written by the unpack, then the
+    # adopted one (index read again)
+    moved_f = (rec_bytes + 4) * n + rec_bytes * m + ((2 * id_bytes + 4) * n + id_bytes * m if ids else 0)
+    print(json.dumps(dict(what="fan_out_unpack", rng=mode, rows=m, envs=n, ms=round(ms, 4), bytes=moved_f, tb_s=round(moved_f / ms / 1e9, 3),
                           frac_datasheet=round(moved_f / ms / 1e-3 / PEAK, 3))))
     del sim, snap, few
 
@@ -108,10 +122,10 @@ def main():
         e = [torch.cuda.Event(enable_timing=True) for _ in range(6)] if record else None
         if record:
             e[0].record()
-        s = plant.snapshot()
+        s = plant.snapshot(rng=ids)
         if record:
             e[1].record()
-        model.restore(s, rows=ridx)
+        model.restore(s, rows=ridx, rng=mode)
         if record:
             e[2].record()
         model.rollout_into(cand, h, 1, None, None, rew, None)
@@ -126,6 +140,17 @@ def main():
             e[5].record()
             marks.append(e)
 
+    if ids:  # common random numbers: the candidates of a plant see one reference trajectory until they terminate
+        model.restore(plant.snapshot(rng=True), rows=ridx, rng="source")
+        _, ref, _, term = model.rollout(cand, record_every=1)
+        ref, term = ref.view(h, p_n, c, -1), term.view(h, p_n, c).bool()
+        alive = term.int().cumsum(0) == 0  # no termination up to and including this step (a terminating step records the ref after its reset)
+        alive = alive & alive[:, :, :1]
+        same = (ref == ref[:, :, :1]).all(-1) | ~alive
+        if not bool(same.all()):
+            raise SystemExit("candidates of one plant recorded different reference trajectories with rng=source")
+        print(json.dumps(dict(what="common_reference_check", plants=p_n, candidates=c, horizon=h, compared_steps=int(alive.sum()), ok=True)))
+
     for _ in range(3):
         control_step()
     torch.cuda.synchronize()
@@ -138,8 +163,45 @@ def main():
         split[lab] = round(v[len(v) // 2], 4)
     tot = sorted(e[0].elapsed_time(e[5]) for e in marks)
     tot_ms = tot[len(tot) // 2]
-    print(json.dumps(dict(what="mpc_control_step", plants=p_n, candidates=c, horizon=h, ms=round(tot_ms, 4), control_steps_per_s=round(1e3 / tot_ms, 1),
+    print(json.dumps(dict(what="mpc_control_step", rng=mode, plants=p_n, candidates=c, horizon=h, ms=round(tot_ms, 4), control_steps_per_s=round(1e3 / tot_ms, 1),
                           env_steps_per_s=round(p_n * c * h / tot_ms * 1e3, 1), split_ms=split)))
+    del plant, model, cand, rew
+    if ids:
+        torch.cuda.empty_cache()
+        print(json.dumps(rollout_arms(n, 32, args.reps)))
+
+
+def rollout_arms(n, steps, reps):
+    """us per env step of a recorded rollout: shared coefficients / per-env blocks of the shared parameters / the same with identities"""
+    arms = {a: sim_of(n, seed=3) for a in ("shared", "envp", "envp_ids")}
+    cfg = arms["envp"].cfg
+    mp = np.tile(np.array(list(cfg.motor_param)), (n, 1))
+    lp = np.tile(np.array(list(cfg.load_param)), (n, 1))
+    arms["envp"].set_env_params(mp, lp)
+    for s in arms.values():
+        s.reset()
+    s = arms["envp_ids"]  # every env adopts the identity of another env of the handle (a rotation): all of them read an identity row
+    s.restore(s.snapshot(rng=True), rows=torch.roll(torch.arange(n, device=s.device, dtype=torch.int32), 1), rng="source")
+    acts = (torch.rand((steps, n, s.n_act), device=s.device, generator=torch.Generator(device=s.device).manual_seed(0)) * 2 - 1).contiguous()
+    for _ in range(3):
+        for s in arms.values():
+            s.rollout(acts, record_every=1)
+    torch.cuda.synchronize()
+    ev = {a: [] for a in arms}
+    for _ in range(reps):
+        for a, s in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            s.rollout(acts, record_every=1)
+            e1.record()
+            ev[a].append((e0, e1))
+    torch.cuda.synchronize()
+    out = dict(what="identity_rollout", env="Cont-CC-PMSM-v0", envs=n, steps=steps, reps=reps, dtype="float32", layout="aos")
+    for a in arms:
+        ms = sorted(x.elapsed_time(y) for x, y in ev[a])
+        out[f"us_per_step_{a}"] = round(ms[len(ms) // 2] * 1e3 / steps, 3)
+    out["envp_ids_over_envp"] = round(out["us_per_step_envp_ids"] / out["us_per_step_envp"], 4)
+    return out
 
 
 if __name__ == "__main__":
