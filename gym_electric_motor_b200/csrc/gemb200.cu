@@ -29,12 +29,17 @@ static int fail(int code, const std::string& msg) { g_last_error = msg; return c
 // ----------------------------------------------------------------------------------------------------------------
 // handle
 // ----------------------------------------------------------------------------------------------------------------
+enum BlockSource {   // per-env parameter blocks of a handle
+  kBlocksNone = 0,   // none: every env uses the shared coefficients
+  kBlocksShared = 1, // the shared parameters, filled by an adoption of RNG identities (which only the ENVP instantiations read)
+  kBlocksCaller = 2  // the caller's: rows of gemb200_set_env_params, or parameter draws
+};
 struct gemb200_handle {
   gemb200_config cfg;
   int fam = 0, n_state = 0, n_ode = 0, n_act = 0, n_ref = 0, nx = 0;
-  bool has_eps = false, any_wiener = false, two_segment = false, any_switched = false;
+  bool has_eps = false, any_wiener = false, two_segment = false;
   size_t rsz = 4;  // sizeof(real)
-  // persistent device state
+  // persistent per-env device state: allocated, freed, saved, reseeded and packed by walking sections()
   int NH = 0, NC = 0;  // words per env in the hot / cold record
   void* d_st = nullptr;
   void* d_stc = nullptr;
@@ -44,20 +49,26 @@ struct gemb200_handle {
   int fifo_dim = 0;
   void* d_sup = nullptr;   // RC supply state [2][n]
   double* d_supph = nullptr;  // AC supply phase [n]
-  void* d_ext = nullptr;       // external speed profile table (real)
   uint32_t* d_kenv = nullptr;  // steps since the reset per env (external speed profile)
   uint32_t* d_swst = nullptr;  // switched reference generators [n_ref][2][n]
   void* d_obsv = nullptr;  // FluxObserver integrator [4][n]: re, im, compensation of re, of im
-  void* d_envp = nullptr;    // per-env model coefficients [kCoefWords][n] (gemb200_set_env_params), nullptr: shared coefficients
-  int plain_shape = 0;       // the configuration has the PLAIN shape (before per-env parameters switch the specialisation off)
+  void* d_imprev = nullptr;  // induction motors with random initial states [2][n]: initial currents of the env's previous episode
+  // other device buffers
+  void* d_ext = nullptr;       // external speed profile table (real)
+  void* d_envp = nullptr;    // per-env model coefficients [kCoefWords][n] (gemb200_set_env_params), allocated at the first use
   double* d_praw = nullptr;  // physical parameters per env [kMaxDraw][n] (double), valid whenever d_envp is in use
   ParamDraw* d_draw = nullptr;  // distributions of the parameters drawn at every reset (gemb200_set_param_randomization)
-  int n_draw = 0;               // parameters drawn per reset (0: none)
-  void* d_imprev = nullptr;  // induction motors with random initial states [2][n]: initial currents of the env's previous episode
   uint32_t* d_rngid = nullptr;  // RNG identities [kRngIdWords][n] (gemb200_adopt_rng_ids), allocated at the first adoption
-  bool ids_adopted = false;     // an identity was adopted since the last reseed / gemb200_clear_rng_ids
+  // launch mode: which instantiation a launch takes (PLAIN, general or ENVP, DESIGN §4).  apply_mode() derives the mode fields of the
+  // live StepParams from these; every entry point that changes one of them calls it.
+  BlockSource blocks = kBlocksNone;  // where the per-env parameter blocks in d_envp / d_praw come from
+  int n_draw = 0;            // parameters drawn per reset (0: none)
+  bool ids_in_use = false;   // adopted RNG identities in d_rngid, since the last reseed / gemb200_clear_rng_ids
+  int n_dst = 0;             // peer destinations of the output stores (gemb200_bind_peers)
+  int64_t dst_delta[8] = {};
+  bool plain_shape = false;  // the configuration has the PLAIN shape (fill_params), which per-env blocks and peer stores switch off
   int n_obs = 0, row_stride = 0;
-  StepParams<float> pf;
+  StepParams<float> pf;      // the parameter block of the handle's dtype is the live one; only with_params() names them
   StepParams<double> pd;
   uint64_t gstep = 0;
   uint64_t n_steps = 0;  // step calls so far (dead-time ring position)
@@ -72,6 +83,31 @@ struct gemb200_handle {
   uint8_t *d_term = nullptr, *d_mask = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 };
+
+// The one dispatch on the handle's dtype: f(the live StepParams<real>).  Inside f, decltype(p.tau) is `real`.
+template <typename F>
+static auto with_params(gemb200_handle* h, F&& f) {
+  if (h->cfg.dtype == GEMB200_F32) return f(h->pf);
+  return f(h->pd);
+}
+// the mode fields of the live StepParams, derived from the handle's launch mode
+static void apply_mode(gemb200_handle* h) {
+  with_params(h, [h](auto& p) {
+    using real = decltype(p.tau);
+    p.envp = h->blocks != kBlocksNone ? static_cast<const real*>(h->d_envp) : nullptr;
+    p.praw = h->d_praw;
+    p.coef_shared = h->blocks == kBlocksShared;
+    p.n_draw = h->n_draw;
+    p.draw = h->d_draw;
+    p.rngid = h->ids_in_use ? h->d_rngid : nullptr;
+    p.n_dst = h->n_dst;
+    std::memcpy(p.dst_delta, h->dst_delta, sizeof(p.dst_delta));
+    // the PLAIN instantiations read the shared constant-bank coefficients and store to the caller's tensors only
+    p.plain = h->plain_shape && h->blocks == kBlocksNone && h->n_dst == 0;
+  });
+}
+// neither checkpoints nor packed rows carry the parameters drawn per reset (DESIGN §7)
+static bool draws_on(const gemb200_handle* h) { return h->n_draw > 0; }
 
 // ----------------------------------------------------------------------------------------------------------------
 // dimensions / validation (SCMLSystem._set_indices physical_systems.py:141-162, :462-485, :594-617, :737-763)
@@ -243,9 +279,10 @@ static bool any_switched_slot(const gemb200_config* c) {
   return false;
 }
 constexpr int kMaxSections = 16;
-// The persistent per-env arrays of a configuration, in checkpoint order.  One table serves the checkpoint blob (ptr, bytes), the reseed
-// and the packed env records of gemb200_pack_envs / gemb200_unpack_envs (element size, elements per env, placement, clock-relative
-// fields), so an array cannot be in one and missing from the other.  h == nullptr: shapes only (ptr = nullptr).
+// The persistent per-env arrays of a configuration, in checkpoint order.  One table serves the allocation at create and the release at
+// destroy (slot: where the handle keeps the array's device pointer, bytes), the checkpoint blob, the reseed and the packed env records of
+// gemb200_pack_envs / gemb200_unpack_envs (element size, elements per env, placement, clock-relative fields), so an array cannot be in
+// one and missing from another.  h == nullptr: shapes only (slot = nullptr).
 // checkpoint blob: [header][hot records][cold records][eps][sw][dead-time queue]...  The header pins the blob to the configuration that
 // wrote it: a blob of equal size from another motor / seed / tau / generator set is refused instead of being reinterpreted.
 enum SecPlace { kPlanar = 0, kRecord = 1 };  // planar: element e of env i at [e * n + i]; record: 16-byte chunked record (word_offset)
@@ -255,35 +292,29 @@ enum SecClock {
   kClkSwst = 2,  // switched generators [n_ref][2]: the super-episode end (odd elements)
   kClkRing = 3   // dead-time ring [dead_time_steps][fifo_dim], stored oldest entry first in a row
 };
-struct Section { void* ptr; size_t bytes; int esz, per_env, place, clk; };  // esz: bytes per element
-static int config_sections(const gemb200_config* c, const gemb200_handle* h, Section* s) {
+struct Section { void** slot; size_t bytes; int esz, per_env, place, clk; };  // esz: bytes per element
+static int config_sections(const gemb200_config* c, gemb200_handle* h, Section* s) {
   Dims d;
   derive_dims(c, &d);
   const size_t n = (size_t)c->n_envs;
   const int rsz = c->dtype == GEMB200_F32 ? 4 : 8;
   int k = 0;
-  auto add = [&](void* p, int esz, int per_env, int place, int clk) { s[k++] = {p, n * (size_t)per_env * esz, esz, per_env, place, clk}; };
-  add(h ? h->d_st : nullptr, rsz, hot_words(d.nx, c->n_ref), kRecord, kClkNone);
-  add(h ? h->d_stc : nullptr, rsz, cold_words(d.nx, c->n_ref), kRecord, kClkCold);
-  if (d.has_eps) add(h ? h->d_eps : nullptr, 8, 1, kPlanar, kClkNone);
-  if (has_sw_state(c)) add(h ? h->d_sw : nullptr, 2, 1, kPlanar, kClkNone);
-  if (c->dead_time_steps > 0) add(h ? h->d_fifo : nullptr, rsz, c->dead_time_steps * fifo_dim_of(c, d), kPlanar, kClkRing);
-  if (d.has_observer) add(h ? h->d_obsv : nullptr, rsz, 4, kPlanar, kClkNone);
-  if (c->supply_kind == GEMB200_SUPPLY_RC) add(h ? h->d_sup : nullptr, rsz, 2, kPlanar, kClkNone);
-  if (c->supply_kind == GEMB200_SUPPLY_AC1) add(h ? h->d_supph : nullptr, 8, 1, kPlanar, kClkNone);
-  if (any_switched_slot(c)) add(h ? h->d_swst : nullptr, 4, 2 * c->n_ref, kPlanar, kClkSwst);
-  if (c->load_kind == GEMB200_LOAD_EXT_SPEED) add(h ? h->d_kenv : nullptr, 4, 1, kPlanar, kClkNone);
-  if (c->init_im_valid) add(h ? h->d_imprev : nullptr, rsz, 2, kPlanar, kClkNone);
+  auto add = [&](void* p, int esz, int per_env, int place, int clk) { s[k++] = {static_cast<void**>(p), n * (size_t)per_env * esz, esz, per_env, place, clk}; };
+  add(h ? &h->d_st : nullptr, rsz, hot_words(d.nx, c->n_ref), kRecord, kClkNone);
+  add(h ? &h->d_stc : nullptr, rsz, cold_words(d.nx, c->n_ref), kRecord, kClkCold);
+  if (d.has_eps) add(h ? &h->d_eps : nullptr, 8, 1, kPlanar, kClkNone);
+  if (has_sw_state(c)) add(h ? &h->d_sw : nullptr, 2, 1, kPlanar, kClkNone);
+  if (c->dead_time_steps > 0) add(h ? &h->d_fifo : nullptr, rsz, c->dead_time_steps * fifo_dim_of(c, d), kPlanar, kClkRing);
+  if (d.has_observer) add(h ? &h->d_obsv : nullptr, rsz, 4, kPlanar, kClkNone);
+  if (c->supply_kind == GEMB200_SUPPLY_RC) add(h ? &h->d_sup : nullptr, rsz, 2, kPlanar, kClkNone);
+  if (c->supply_kind == GEMB200_SUPPLY_AC1) add(h ? &h->d_supph : nullptr, 8, 1, kPlanar, kClkNone);
+  if (any_switched_slot(c)) add(h ? &h->d_swst : nullptr, 4, 2 * c->n_ref, kPlanar, kClkSwst);
+  if (c->load_kind == GEMB200_LOAD_EXT_SPEED) add(h ? &h->d_kenv : nullptr, 4, 1, kPlanar, kClkNone);
+  if (c->init_im_valid) add(h ? &h->d_imprev : nullptr, rsz, 2, kPlanar, kClkNone);
   return k;  // (the per-env parameter table is configuration, not state: re-apply gemb200_set_env_params after a load; parameter draws
              //  per reset make it state, so checkpoints and snapshots are refused while they are on)
 }
 static int sections(gemb200_handle* h, Section* s) { return config_sections(&h->cfg, h, s); }
-static bool sections_allocated(gemb200_handle* h) {
-  Section s[kMaxSections];
-  const int k = sections(h, s);
-  for (int q = 0; q < k; ++q) if (!s[q].ptr) return false;
-  return true;
-}
 static int row_words(const Section& s) { return s.per_env * (s.esz == 8 ? 2 : 1); }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -369,14 +400,21 @@ static void derive_model(const gemb200_config* cfg, const Dims& dm, Derived* o) 
 }
 
 template <typename real>
-static void fill_params(const gemb200_handle* h, const Dims& dm, const Derived& dv, StepParams<real>* p) {
+static void set_seed(StepParams<real>* p, uint64_t seed) {
+  p->seed_lo = (uint32_t)seed; p->seed_hi = (uint32_t)(seed >> 32);
+  for (int r = 0; r < 10; ++r) { p->rk[r][0] = p->seed_lo + (uint32_t)r * 0x9E3779B9u; p->rk[r][1] = p->seed_hi + (uint32_t)r * 0xBB67AE85u; }
+}
+
+// fills the parameter block of a fresh handle (launch mode off: apply_mode() sets those fields); returns whether the configuration has the
+// PLAIN shape
+template <typename real>
+static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& dv, StepParams<real>* p) {
   const gemb200_config& c = h->cfg;
   std::memset(p, 0, sizeof(*p));
   p->n = c.n_envs;
   p->env_begin = 0; p->env_end = c.n_envs;
   p->env_offset = c.env_index_offset;
-  p->seed_lo = (uint32_t)c.seed; p->seed_hi = (uint32_t)(c.seed >> 32);
-  for (int r = 0; r < 10; ++r) { p->rk[r][0] = p->seed_lo + (uint32_t)r * 0x9E3779B9u; p->rk[r][1] = p->seed_hi + (uint32_t)r * 0xBB67AE85u; }
+  set_seed(p, c.seed);
   p->st = static_cast<real*>(h->d_st);
   p->stc = static_cast<real*>(h->d_stc);
   p->kstep = 0;
@@ -500,6 +538,7 @@ static void fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
   for (int r = 0; r < kMaxRef; ++r) if (p->rwr_w[r] == real(0)) p->rwr_pow1[r] = 1;  // unused slots: no pow()
   p->bias = (real)c.reward_bias; p->viol_reward = (real)c.violation_reward;
   // PLAIN shape (step_kernel): decided here once; GEMB200_NO_PLAIN=1 in the environment forces the general instantiation (A/B runs)
+  bool plain_shape;
   {
     bool plain =
                  c.load_kind != GEMB200_LOAD_EXT_SPEED && c.supply_kind == GEMB200_SUPPLY_IDEAL && (c.finite || (c.interlocking_time == 0.0 && !(c.interlocking_time1 > 0.0))) && c.dead_time_steps == 0 && !c.action_dq && c.n_state_ops == 0 &&
@@ -513,8 +552,7 @@ static void fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
     for (int q = 0; q < 2; ++q) p->mon_off[2 + q] = (p->n_sq > 0 && p->sq_cnt[0] == 2) ? p->sq_idx[0][q] * (int)sizeof(real) : 0;
     p->mon_thr[2] = p->n_sq > 0 ? real(1) : inf;
     const char* off = std::getenv("GEMB200_NO_PLAIN");
-    p->plain = plain && !(off && off[0] == '1');
-    const_cast<gemb200_handle*>(h)->plain_shape = p->plain;
+    plain_shape = plain && !(off && off[0] == '1');
   }
   {  // L2 prefetch distance: one wave of resident threads (SMs x blocks/SM x block size); GEMB200_PF_DIST overrides (0 = off)
     int sms = 132;  // H100 SXM; the attribute query below gives the real count
@@ -577,6 +615,7 @@ static void fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
     }
     p->ref_len_lo[r] = c.ref_len_lo[r]; p->ref_len_span[r] = c.ref_len_hi[r] - c.ref_len_lo[r];
   }
+  return plain_shape;
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -673,24 +712,15 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
   const uint64_t g0 = h->gstep - (ksteps - 1), n0 = h->n_steps - (ksteps - 1);  // call id / step count of the FIRST step of this launch
   if (end < 0) end = h->cfg.n_envs;
   const int fifo_slot = h->cfg.dead_time_steps > 0 ? (int)((n0 - 1) % (uint64_t)h->cfg.dead_time_steps) : 0;
-  cudaError_t e;
-  if (h->cfg.dtype == GEMB200_F32) {
-    StepParams<float>& p = h->pf;
+  const cudaError_t e = with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
     p.env_begin = begin; p.env_end = end; p.fifo_slot = fifo_slot; p.kstep = dev_clock ? 1u : (uint32_t)n0;
     p.gstep_lo = (uint32_t)g0; p.gstep_hi = (uint32_t)(g0 >> 32); p.clock_dev = dev_clock ? h->d_clock : nullptr;
     p.roll_steps = roll; p.record_every = every;
-    p.action = action; p.obs = (float*)obs; p.ref_out = (float*)ref; p.reward = (float*)rew; p.term = term;
+    p.action = action; p.obs = (real*)obs; p.ref_out = (real*)ref; p.reward = (real*)rew; p.term = term;
     set_roll_strides(h, p);
-    e = launch_step<float>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
-  } else {
-    StepParams<double>& p = h->pd;
-    p.env_begin = begin; p.env_end = end; p.fifo_slot = fifo_slot; p.kstep = dev_clock ? 1u : (uint32_t)n0;
-    p.gstep_lo = (uint32_t)g0; p.gstep_hi = (uint32_t)(g0 >> 32); p.clock_dev = dev_clock ? h->d_clock : nullptr;
-    p.roll_steps = roll; p.record_every = every;
-    p.action = action; p.obs = (double*)obs; p.ref_out = (double*)ref; p.reward = (double*)rew; p.term = term;
-    set_roll_strides(h, p);
-    e = launch_step<double>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
-  }
+    return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
+  });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string(roll > 0 ? "rollout launch: " : "step launch: ") + cudaGetErrorString(e));
   h->launches += 1;
   // (the alternative is to advance the clock from the step kernel itself — its last block to finish, one atomic per block; at N = 65 536 the
@@ -702,21 +732,15 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
 static int do_reset(gemb200_handle* h, const uint8_t* mask, void* obs, void* ref, cudaStream_t st) {
   const bool dev_clock = h->dev_clock;
   if (!dev_clock) h->gstep += 1;
-  h->pf.clock_dev = h->pd.clock_dev = dev_clock ? h->d_clock : nullptr;
-  cudaError_t e;
-  if (h->cfg.dtype == GEMB200_F32) {
-    StepParams<float>& p = h->pf;
+  const cudaError_t e = with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    p.clock_dev = dev_clock ? h->d_clock : nullptr;
     p.gstep_lo = (uint32_t)h->gstep; p.gstep_hi = (uint32_t)(h->gstep >> 32);
-    p.reset_mask = mask; p.obs = (float*)obs; p.ref_out = (float*)ref; p.kstep = dev_clock ? 0u : (uint32_t)h->n_steps;
-    e = launch_reset<float>(h->fam, h->n_ref, p, st);
+    p.reset_mask = mask; p.obs = (real*)obs; p.ref_out = (real*)ref; p.kstep = dev_clock ? 0u : (uint32_t)h->n_steps;
+    const cudaError_t le = launch_reset<real>(h->fam, h->n_ref, p, st);
     p.reset_mask = nullptr;
-  } else {
-    StepParams<double>& p = h->pd;
-    p.gstep_lo = (uint32_t)h->gstep; p.gstep_hi = (uint32_t)(h->gstep >> 32);
-    p.reset_mask = mask; p.obs = (double*)obs; p.ref_out = (double*)ref; p.kstep = dev_clock ? 0u : (uint32_t)h->n_steps;
-    e = launch_reset<double>(h->fam, h->n_ref, p, st);
-    p.reset_mask = nullptr;
-  }
+    return le;
+  });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string("reset launch: ") + cudaGetErrorString(e));
   h->launches += 1;
   if (dev_clock) return tick_clock(h, 1u, 0u, st);
@@ -727,18 +751,14 @@ static int do_reset(gemb200_handle* h, const uint8_t* mask, void* obs, void* ref
 static int fill_imprev(gemb200_handle* h, cudaStream_t st) {
   if (!h->d_imprev) return GEMB200_OK;
   const size_t n = (size_t)h->cfg.n_envs;
-  if (h->cfg.dtype == GEMB200_F32) {
-    std::vector<float> v(2 * n);
-    for (size_t q = 0; q < n; ++q) { v[q] = (float)h->cfg.init_ode[1]; v[n + q] = (float)h->cfg.init_ode[2]; }
-    CUDA_TRY(cudaMemcpyAsync(h->d_imprev, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+  return with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    std::vector<real> v(2 * n);
+    for (size_t q = 0; q < n; ++q) { v[q] = (real)h->cfg.init_ode[1]; v[n + q] = (real)h->cfg.init_ode[2]; }
+    CUDA_TRY(cudaMemcpyAsync(h->d_imprev, v.data(), v.size() * sizeof(real), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-  } else {
-    std::vector<double> v(2 * n);
-    for (size_t q = 0; q < n; ++q) { v[q] = h->cfg.init_ode[1]; v[n + q] = h->cfg.init_ode[2]; }
-    CUDA_TRY(cudaMemcpyAsync(h->d_imprev, v.data(), v.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-  }
-  return GEMB200_OK;
+    return GEMB200_OK;
+  });
 }
 
 struct DeviceGuard {
@@ -746,6 +766,17 @@ struct DeviceGuard {
   explicit DeviceGuard(int dev) { cudaGetDevice(&prev); if (prev != dev) cudaSetDevice(dev); else prev = -1; }
   ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
+
+// one launch of an ODE-state / reference accessor kernel over every env: launch(live StepParams, n, grid, stream)
+template <typename F>
+static int launch_accessor(gemb200_handle* h, void* stream, F&& launch) {
+  DeviceGuard guard(h->cfg.device);
+  const int n = h->cfg.n_envs, grid = (n + 255) / 256;
+  with_params(h, [&](auto& p) { launch(p, n, grid, (cudaStream_t)stream); });
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return GEMB200_OK;
+}
 
 // ----------------------------------------------------------------------------------------------------------------
 // C-ABI
@@ -811,35 +842,24 @@ int gemb200_create(const gemb200_config* cfg, gemb200_handle** out) {
     bool used = r < cfg->n_ref;
     for (int q = 0; q < cfg->n_ref; ++q) used = used || (cfg->ref_sw_count[q] > 1 && r >= cfg->ref_sw_first[q] && r < cfg->ref_sw_first[q] + cfg->ref_sw_count[q]);
     if (used) h->any_wiener = h->any_wiener || cfg->ref_kind[r] == GEMB200_REF_WIENER || cfg->ref_kind[r] >= GEMB200_REF_LAPLACE;
-    if (r < cfg->n_ref && cfg->ref_sw_count[r] > 1) h->any_switched = true;
   }
-  const size_t n = (size_t)cfg->n_envs;
-#define ALLOC(ptr, bytes)                                                                                     \
-  do {                                                                                                        \
-    cudaError_t e_ = cudaMalloc((void**)&(ptr), (bytes));                                                     \
-    if (e_ != cudaSuccess) { gemb200_destroy(h); return fail(e_ == cudaErrorMemoryAllocation ? GEMB200_E_NOMEM : GEMB200_E_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e_)); } \
-    cudaMemset((ptr), 0, (bytes));                                                                            \
-  } while (0)
   h->NH = hot_words(d.nx, cfg->n_ref); h->NC = cold_words(d.nx, cfg->n_ref);
-  ALLOC(h->d_st, n * (h->NH > 0 ? h->NH : 1) * h->rsz);
-  ALLOC(h->d_stc, n * h->NC * h->rsz);
-  if (cfg->dead_time_steps > 0) {
-    h->fifo_dim = fifo_dim_of(cfg, d);
-    ALLOC(h->d_fifo, n * cfg->dead_time_steps * h->fifo_dim * h->rsz);
+  h->fifo_dim = fifo_dim_of(cfg, d);
+  {  // every per-env array, zero-filled, then the speed-profile table
+    Section s[kMaxSections];
+    const int k = sections(h, s);
+    cudaError_t e = cudaSuccess;
+    for (int q = 0; q < k && e == cudaSuccess; ++q)
+      if ((e = cudaMalloc(s[q].slot, s[q].bytes)) == cudaSuccess) cudaMemset(*s[q].slot, 0, s[q].bytes);
+    if (e == cudaSuccess && cfg->load_kind == GEMB200_LOAD_EXT_SPEED) e = cudaMalloc(&h->d_ext, (size_t)cfg->ext_speed_len * h->rsz);
+    if (e != cudaSuccess) { gemb200_destroy(h); return fail(e == cudaErrorMemoryAllocation ? GEMB200_E_NOMEM : GEMB200_E_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e)); }
   }
-  if (d.has_eps) ALLOC(h->d_eps, n * sizeof(double));
-  if (has_sw_state(cfg)) ALLOC(h->d_sw, n * sizeof(uint16_t));
-  if (cfg->supply_kind == GEMB200_SUPPLY_RC) ALLOC(h->d_sup, n * 2 * h->rsz);
-  if (cfg->supply_kind == GEMB200_SUPPLY_AC1) ALLOC(h->d_supph, n * sizeof(double));
   if (cfg->load_kind == GEMB200_LOAD_EXT_SPEED) {
-    ALLOC(h->d_kenv, n * sizeof(uint32_t));
-    ALLOC(h->d_ext, (size_t)cfg->ext_speed_len * h->rsz);
-    if (cfg->dtype == GEMB200_F32) {
-      std::vector<float> tmp(cfg->ext_speed_table, cfg->ext_speed_table + cfg->ext_speed_len);
-      cudaMemcpy(h->d_ext, tmp.data(), tmp.size() * sizeof(float), cudaMemcpyHostToDevice);
-    } else {
-      cudaMemcpy(h->d_ext, cfg->ext_speed_table, (size_t)cfg->ext_speed_len * sizeof(double), cudaMemcpyHostToDevice);
-    }
+    with_params(h, [&](auto& p) {
+      using real = decltype(p.tau);
+      std::vector<real> tmp(cfg->ext_speed_table, cfg->ext_speed_table + cfg->ext_speed_len);
+      cudaMemcpy(h->d_ext, tmp.data(), tmp.size() * sizeof(real), cudaMemcpyHostToDevice);
+    });
     {
       uint64_t x = 1469598103934665603ull;
       const unsigned char* tb = reinterpret_cast<const unsigned char*>(cfg->ext_speed_table);
@@ -848,11 +868,6 @@ int gemb200_create(const gemb200_config* cfg, gemb200_handle** out) {
     }
     h->cfg.ext_speed_table = nullptr;  // the caller's buffer is not referenced after create
   }
-  if (h->any_switched) ALLOC(h->d_swst, n * 2 * cfg->n_ref * sizeof(uint32_t));
-  if (d.has_observer) ALLOC(h->d_obsv, n * 4 * h->rsz);
-  if (cfg->init_im_valid) ALLOC(h->d_imprev, n * 2 * h->rsz);
-#undef ALLOC
-  if (!sections_allocated(h)) { gemb200_destroy(h); return fail(GEMB200_E_INVALID, "internal: a per-env array of the section table is not allocated"); }
   Derived dv;
   derive_model(cfg, d, &dv);
   {  // same derivation one volt higher: the difference is the u_sup-proportional part of the reset observation
@@ -862,8 +877,8 @@ int gemb200_create(const gemb200_config* cfg, gemb200_handle** out) {
     derive_model(&c1, d, &dv1);
     for (int j = 0; j < d.n_state; ++j) dv.reset_obs_du[j] = dv1.reset_obs[j] - dv.reset_obs[j];
   }
-  fill_params<float>(h, d, dv, &h->pf);
-  fill_params<double>(h, d, dv, &h->pd);
+  h->plain_shape = with_params(h, [&](auto& p) { return fill_params(h, d, dv, &p); });
+  apply_mode(h);
   cudaEventCreate(&h->ev0);
   cudaEventCreate(&h->ev1);
   rc = fill_imprev(h, nullptr);
@@ -879,8 +894,9 @@ int gemb200_create(const gemb200_config* cfg, gemb200_handle** out) {
 int gemb200_destroy(gemb200_handle* h) {
   if (!h) return GEMB200_OK;
   DeviceGuard guard(h->cfg.device);
-  cudaFree(h->d_st); cudaFree(h->d_stc); cudaFree(h->d_eps); cudaFree(h->d_sw); cudaFree(h->d_fifo); cudaFree(h->d_obsv); cudaFree(h->d_sup); cudaFree(h->d_supph); cudaFree(h->d_swst); cudaFree(h->d_ext); cudaFree(h->d_kenv); cudaFree(h->d_imprev); cudaFree(h->d_envp); cudaFree(h->d_clock);
-  cudaFree(h->d_praw); cudaFree(h->d_draw); cudaFree(h->d_rngid);
+  Section s[kMaxSections];
+  for (int q = 0, ns = sections(h, s); q < ns; ++q) cudaFree(*s[q].slot);
+  cudaFree(h->d_ext); cudaFree(h->d_envp); cudaFree(h->d_clock); cudaFree(h->d_praw); cudaFree(h->d_draw); cudaFree(h->d_rngid);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_ref); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_mask);
   if (h->hstream) cudaStreamDestroy(h->hstream);
   for (int k = 0; k < 3; ++k) if (h->hpipe[k]) cudaStreamDestroy(h->hpipe[k]);
@@ -928,16 +944,16 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   if (h->cfg.layout != GEMB200_LAYOUT_AOS && (motor_param || load_param))
     return fail(GEMB200_E_INVALID, "per-env parameter blocks need the row-per-env (AoS) I/O layout");
   if (!motor_param && !load_param) {
-    h->n_draw = 0; h->pf.n_draw = 0; h->pd.n_draw = 0;  // shared coefficients again: no parameter draws either
-    if (h->pf.rngid) {  // adopted RNG identities are read by the ENVP instantiations only: the blocks take the shared parameters instead
-      const int rc = fill_shared_blocks(h);
-      if (rc) return rc;
-      h->pf.coef_shared = h->pd.coef_shared = 1;
-      return GEMB200_OK;
+    h->n_draw = 0;  // shared coefficients again: no parameter draws either
+    int rc = GEMB200_OK;
+    if (h->ids_in_use) {  // adopted RNG identities are read by the ENVP instantiations only: the blocks take the shared parameters instead
+      rc = fill_shared_blocks(h);
+      if (!rc) h->blocks = kBlocksShared;
+    } else {
+      h->blocks = kBlocksNone;
     }
-    h->pf.envp = nullptr; h->pd.envp = nullptr;
-    h->pf.plain = h->pf.n_dst == 0 ? h->plain_shape : 0; h->pd.plain = h->pf.plain;
-    return GEMB200_OK;
+    apply_mode(h);
+    return rc;
   }
   const size_t n = (size_t)h->cfg.n_envs;
   Dims d;
@@ -963,16 +979,15 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, tab.size() * h->rsz));
   if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, raw.size() * sizeof(double)));
   CUDA_TRY(cudaMemcpy(h->d_praw, raw.data(), raw.size() * sizeof(double), cudaMemcpyHostToDevice));
-  if (h->cfg.dtype == GEMB200_F32) {
-    std::vector<float> tf(tab.begin(), tab.end());
-    CUDA_TRY(cudaMemcpy(h->d_envp, tf.data(), tf.size() * sizeof(float), cudaMemcpyHostToDevice));
-  } else {
-    CUDA_TRY(cudaMemcpy(h->d_envp, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice));
-  }
-  h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
-  h->pf.plain = 0; h->pd.plain = 0;  // the PLAIN instantiations read the shared constant-bank coefficients
-  h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
-  h->pf.coef_shared = h->pd.coef_shared = 0;
+  const int rc = with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    const std::vector<real> t(tab.begin(), tab.end());
+    CUDA_TRY(cudaMemcpy(h->d_envp, t.data(), t.size() * sizeof(real), cudaMemcpyHostToDevice));
+    return GEMB200_OK;
+  });
+  if (rc) return rc;
+  h->blocks = kBlocksCaller;
+  apply_mode(h);
   return GEMB200_OK;
 }
 
@@ -995,15 +1010,11 @@ __global__ void fill_env_params_kernel(real* envp, double* praw, const Coef<real
 // no adopted identities any more: launches key every env by its own identity again, and blocks that only an adoption made go, so that the
 // handle runs its shared-coefficient kernels like a fresh one (the identity array stays allocated for the next adoption)
 static void drop_rng_ids(gemb200_handle* h) {
-  h->pf.rngid = h->pd.rngid = nullptr;
-  h->ids_adopted = false;
-  if (h->pf.coef_shared) {
-    h->pf.envp = nullptr; h->pd.envp = nullptr;
-    h->pf.plain = h->pf.n_dst == 0 ? h->plain_shape : 0; h->pd.plain = h->pf.plain;
-    h->pf.coef_shared = h->pd.coef_shared = 0;
-  }
+  h->ids_in_use = false;
+  if (h->blocks == kBlocksShared) h->blocks = kBlocksNone;
+  apply_mode(h);
 }
-// every env's block := the shared parameters (synchronises); the handle runs its ENVP instantiations from then on
+// every env's block := the shared parameters (synchronises); the caller sets the handle's blocks and applies the mode
 static int fill_shared_blocks(gemb200_handle* h) {
   const size_t nn = (size_t)h->cfg.n_envs;
   if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
@@ -1012,13 +1023,12 @@ static int fill_shared_blocks(gemb200_handle* h) {
   for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
   for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
   const int grid = (int)((nn + 255) / 256);
-  if (h->cfg.dtype == GEMB200_F32) fill_env_params_kernel<float><<<grid, 256>>>(static_cast<float*>(h->d_envp), h->d_praw, h->pf.k, raw, (int)nn);
-  else fill_env_params_kernel<double><<<grid, 256>>>(static_cast<double*>(h->d_envp), h->d_praw, h->pd.k, raw, (int)nn);
+  with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    fill_env_params_kernel<real><<<grid, 256>>>(static_cast<real*>(h->d_envp), h->d_praw, p.k, raw, (int)nn);
+  });
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
-  h->pf.envp = static_cast<const float*>(h->d_envp); h->pd.envp = static_cast<const double*>(h->d_envp);
-  h->pf.plain = 0; h->pd.plain = 0;
-  h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
   return GEMB200_OK;
 }
 // out[j][i] = stored value of drawn parameter j of env i, in the handle's dtype
@@ -1038,7 +1048,8 @@ int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t*
   DeviceGuard guard(h->cfg.device);
   CUDA_TRY(cudaDeviceSynchronize());
   if (n == 0) {  // no more draws; the envs keep their last values
-    h->n_draw = 0; h->pf.n_draw = 0; h->pd.n_draw = 0;
+    h->n_draw = 0;
+    apply_mode(h);
     return GEMB200_OK;
   }
   if (h->cfg.layout != GEMB200_LAYOUT_AOS) return fail(GEMB200_E_INVALID, "parameter draws need the row-per-env (AoS) I/O layout (per-env parameter blocks)");
@@ -1064,25 +1075,25 @@ int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t*
   }
   if (!h->d_draw) CUDA_TRY(cudaMalloc(&h->d_draw, sizeof(ParamDraw)));
   CUDA_TRY(cudaMemcpy(h->d_draw, &pd, sizeof(pd), cudaMemcpyHostToDevice));
-  if (!h->pf.envp) {  // no per-env blocks yet: every env starts from the shared parameters
+  if (h->blocks == kBlocksNone) {  // no per-env blocks yet: every env starts from the shared parameters
     const int rc = fill_shared_blocks(h);
     if (rc) return rc;
   }
-  h->pf.coef_shared = h->pd.coef_shared = 0;  // the draws change the blocks: they are the caller's from now on
+  h->blocks = kBlocksCaller;  // the draws change the blocks: they are the caller's from now on
   h->n_draw = n;
-  h->pf.n_draw = n; h->pd.n_draw = n;
-  h->pf.draw = h->d_draw; h->pd.draw = h->d_draw;
-  h->pf.praw = h->d_praw; h->pd.praw = h->d_praw;
+  apply_mode(h);
   return GEMB200_OK;
 }
 
 int gemb200_get_env_params(gemb200_handle* h, void* out, void* stream) {
   if (!h || !out) return fail(GEMB200_E_INVALID, "NULL argument");
-  if (h->n_draw == 0) return fail(GEMB200_E_INVALID, "no parameters are drawn (gemb200_set_param_randomization)");
+  if (!draws_on(h)) return fail(GEMB200_E_INVALID, "no parameters are drawn (gemb200_set_param_randomization)");
   DeviceGuard guard(h->cfg.device);
   const int n = h->cfg.n_envs, grid = (n + 255) / 256;
-  if (h->cfg.dtype == GEMB200_F32) get_env_params_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(h->d_praw, h->d_draw, h->n_draw, static_cast<float*>(out), n);
-  else get_env_params_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>(h->d_praw, h->d_draw, h->n_draw, static_cast<double*>(out), n);
+  with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    get_env_params_kernel<real><<<grid, 256, 0, (cudaStream_t)stream>>>(h->d_praw, h->d_draw, h->n_draw, static_cast<real*>(out), n);
+  });
   CUDA_TRY(cudaGetLastError());
   return GEMB200_OK;
 }
@@ -1147,11 +1158,9 @@ int gemb200_bind_peers(gemb200_handle* h, int32_t n_dst, const int64_t* dst_delt
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (n_dst < 0 || n_dst > 8 || (n_dst > 0 && !dst_delta)) return fail(GEMB200_E_INVALID, "n_dst must be in [0, 8]");
   if (n_dst > 0 && h->cfg.layout != GEMB200_LAYOUT_AOS) return fail(GEMB200_E_INVALID, "peer destinations need the row-per-env (AoS) layout");
-  h->pf.n_dst = n_dst; h->pd.n_dst = n_dst;
-  for (int d = 0; d < n_dst; ++d) { h->pf.dst_delta[d] = dst_delta[d]; h->pd.dst_delta[d] = dst_delta[d]; }
-  // the PLAIN instantiations store to the caller's tensors only
-  h->pf.plain = (n_dst == 0 && !h->pf.envp) ? h->plain_shape : 0;
-  h->pd.plain = h->pf.plain;
+  h->n_dst = n_dst;
+  for (int d = 0; d < n_dst; ++d) h->dst_delta[d] = dst_delta[d];
+  apply_mode(h);
   return GEMB200_OK;
 }
 int gemb200_peer_signal(gemb200_handle* h, int32_t n_dst, uint32_t* const* flag_ptrs_dev, uint32_t value, void* stream) {
@@ -1251,45 +1260,33 @@ int gemb200_reset_host(gemb200_handle* h, const uint8_t* reset_mask, void* obs_o
 
 int gemb200_get_ode_state(gemb200_handle* h, double* ode_out, void* stream) {
   if (!h || !ode_out) return fail(GEMB200_E_INVALID, "NULL argument");
-  DeviceGuard guard(h->cfg.device);
-  const int n = h->cfg.n_envs, grid = (n + 255) / 256;
-  if (h->cfg.dtype == GEMB200_F32) get_ode_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)h->d_st, (const float*)h->d_stc, h->d_eps, ode_out, n, h->nx, h->n_ref, h->has_eps);
-  else get_ode_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>((const double*)h->d_st, (const double*)h->d_stc, h->d_eps, ode_out, n, h->nx, h->n_ref, h->has_eps);
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 1;
-  return GEMB200_OK;
+  return launch_accessor(h, stream, [&](auto& p, int n, int grid, cudaStream_t st) {
+    using real = decltype(p.tau);
+    get_ode_kernel<real><<<grid, 256, 0, st>>>((const real*)h->d_st, (const real*)h->d_stc, h->d_eps, ode_out, n, h->nx, h->n_ref, h->has_eps);
+  });
 }
 int gemb200_set_ode_state(gemb200_handle* h, const double* ode_in, void* stream) {
   if (!h || !ode_in) return fail(GEMB200_E_INVALID, "NULL argument");
-  DeviceGuard guard(h->cfg.device);
-  const int n = h->cfg.n_envs, grid = (n + 255) / 256;
-  if (h->cfg.dtype == GEMB200_F32) set_ode_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((float*)h->d_st, (float*)h->d_stc, h->d_eps, ode_in, n, h->nx, h->n_ref, h->has_eps);
-  else set_ode_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>((double*)h->d_st, (double*)h->d_stc, h->d_eps, ode_in, n, h->nx, h->n_ref, h->has_eps);
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 1;
-  return GEMB200_OK;
+  return launch_accessor(h, stream, [&](auto& p, int n, int grid, cudaStream_t st) {
+    using real = decltype(p.tau);
+    set_ode_kernel<real><<<grid, 256, 0, st>>>((real*)h->d_st, (real*)h->d_stc, h->d_eps, ode_in, n, h->nx, h->n_ref, h->has_eps);
+  });
 }
 int gemb200_get_reference(gemb200_handle* h, double* ref_out, void* stream) {
   if (!h || !ref_out) return fail(GEMB200_E_INVALID, "NULL argument");
   if (h->n_ref == 0) return GEMB200_OK;
-  DeviceGuard guard(h->cfg.device);
-  const int n = h->cfg.n_envs, grid = (n + 255) / 256;
-  if (h->cfg.dtype == GEMB200_F32) get_ref_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)h->d_st, ref_out, n, h->nx, h->n_ref);
-  else get_ref_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>((const double*)h->d_st, ref_out, n, h->nx, h->n_ref);
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 1;
-  return GEMB200_OK;
+  return launch_accessor(h, stream, [&](auto& p, int n, int grid, cudaStream_t st) {
+    using real = decltype(p.tau);
+    get_ref_kernel<real><<<grid, 256, 0, st>>>((const real*)h->d_st, ref_out, n, h->nx, h->n_ref);
+  });
 }
 int gemb200_set_reference(gemb200_handle* h, const double* ref_in, void* stream) {
   if (!h || !ref_in) return fail(GEMB200_E_INVALID, "NULL argument");
   if (h->n_ref == 0) return GEMB200_OK;
-  DeviceGuard guard(h->cfg.device);
-  const int n = h->cfg.n_envs, grid = (n + 255) / 256;
-  if (h->cfg.dtype == GEMB200_F32) set_ref_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((float*)h->d_st, ref_in, n, h->nx, h->n_ref);
-  else set_ref_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>((double*)h->d_st, ref_in, n, h->nx, h->n_ref);
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 1;
-  return GEMB200_OK;
+  return launch_accessor(h, stream, [&](auto& p, int n, int grid, cudaStream_t st) {
+    using real = decltype(p.tau);
+    set_ref_kernel<real><<<grid, 256, 0, st>>>((real*)h->d_st, ref_in, n, h->nx, h->n_ref);
+  });
 }
 
 struct CheckpointHeader {
@@ -1313,7 +1310,7 @@ static void make_header(gemb200_handle* h, CheckpointHeader* hd) {
   std::memset(hd, 0, sizeof(*hd));
   std::memcpy(hd->magic, "GEMB200C", 8);
   hd->abi = GEMB200_ABI_VERSION; hd->dtype = h->cfg.dtype; hd->n_envs = h->cfg.n_envs; hd->nh = h->NH; hd->nc = h->NC;
-  Section s[16];
+  Section s[kMaxSections];
   hd->n_sections = sections(h, s);
   for (int i = 0; i < hd->n_sections; ++i) hd->payload_bytes += s[i].bytes;
   hd->config_hash = config_hash(h);
@@ -1327,8 +1324,8 @@ int64_t gemb200_checkpoint_size(gemb200_handle* h) {
 }
 int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob) {
   if (!h || !host_blob) return fail(GEMB200_E_INVALID, "NULL argument");
-  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
-  if (h->ids_adopted) return fail(GEMB200_E_INVALID, "checkpoints do not carry adopted RNG identities; clear them first (gemb200_clear_rng_ids, DESIGN §7)");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  if (h->ids_in_use) return fail(GEMB200_E_INVALID, "checkpoints do not carry adopted RNG identities; clear them first (gemb200_clear_rng_ids, DESIGN §7)");
   DeviceGuard guard(h->cfg.device);
   CUDA_TRY(cudaDeviceSynchronize());
   if (h->dev_clock) { int rc = pull_clock(h, nullptr); if (rc) return rc; }  // the header carries the clock
@@ -1336,15 +1333,15 @@ int gemb200_checkpoint_save(gemb200_handle* h, void* host_blob) {
   CheckpointHeader hd;
   make_header(h, &hd);
   std::memcpy(b, &hd, sizeof(hd)); b += sizeof(hd);
-  Section s[16];
+  Section s[kMaxSections];
   const int k = sections(h, s);
-  for (int i = 0; i < k; ++i) { CUDA_TRY(cudaMemcpy(b, s[i].ptr, s[i].bytes, cudaMemcpyDeviceToHost)); b += s[i].bytes; }
+  for (int i = 0; i < k; ++i) { CUDA_TRY(cudaMemcpy(b, *s[i].slot, s[i].bytes, cudaMemcpyDeviceToHost)); b += s[i].bytes; }
   return GEMB200_OK;
 }
 int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob) {
   if (!h || !host_blob) return fail(GEMB200_E_INVALID, "NULL argument");
-  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
-  if (h->ids_adopted) return fail(GEMB200_E_INVALID, "checkpoints do not carry adopted RNG identities; clear them first (gemb200_clear_rng_ids, DESIGN §7)");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "checkpoints do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  if (h->ids_in_use) return fail(GEMB200_E_INVALID, "checkpoints do not carry adopted RNG identities; clear them first (gemb200_clear_rng_ids, DESIGN §7)");
   DeviceGuard guard(h->cfg.device);
   CheckpointHeader want, got;
   make_header(h, &want);
@@ -1359,9 +1356,9 @@ int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob) {
   CUDA_TRY(cudaDeviceSynchronize());
   const char* b = (const char*)host_blob + sizeof(got);
   h->gstep = got.gstep; h->n_steps = got.n_steps;
-  Section s[16];
+  Section s[kMaxSections];
   const int k = sections(h, s);
-  for (int i = 0; i < k; ++i) { CUDA_TRY(cudaMemcpy(s[i].ptr, b, s[i].bytes, cudaMemcpyHostToDevice)); b += s[i].bytes; }
+  for (int i = 0; i < k; ++i) { CUDA_TRY(cudaMemcpy(*s[i].slot, b, s[i].bytes, cudaMemcpyHostToDevice)); b += s[i].bytes; }
   if (h->dev_clock) { int rc = push_clock(h, nullptr); if (rc) return rc; CUDA_TRY(cudaDeviceSynchronize()); }
   return GEMB200_OK;
 }
@@ -1376,16 +1373,12 @@ int gemb200_reseed(gemb200_handle* h, uint64_t seed, void* stream) {
   h->cfg.seed = seed;
   h->gstep = 0; h->n_steps = 0;
   if (h->dev_clock) { int rc = push_clock(h, st); if (rc) return rc; }
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t lo = (uint32_t)seed + (uint32_t)r * 0x9E3779B9u, hi = (uint32_t)(seed >> 32) + (uint32_t)r * 0xBB67AE85u;
-    h->pf.rk[r][0] = lo; h->pf.rk[r][1] = hi; h->pd.rk[r][0] = lo; h->pd.rk[r][1] = hi;
-  }
-  h->pf.seed_lo = h->pd.seed_lo = (uint32_t)seed; h->pf.seed_hi = h->pd.seed_hi = (uint32_t)(seed >> 32);
+  with_params(h, [&](auto& p) { set_seed(&p, seed); });
   drop_rng_ids(h);  // every env draws with its own identity again
-  Section s[16];
+  Section s[kMaxSections];
   const int k = sections(h, s);
   for (int i = 0; i < k; ++i) {
-    CUDA_TRY(cudaMemsetAsync(s[i].ptr, 0, s[i].bytes, st));
+    CUDA_TRY(cudaMemsetAsync(*s[i].slot, 0, s[i].bytes, st));
   }
   int rc = fill_imprev(h, st);
   if (rc) return rc;
@@ -1648,7 +1641,7 @@ static void record_args(gemb200_handle* h, RecArgs* a) {
   int off = 0;
   a->swst_off = -1;
   for (int q = 0; q < k; ++q) {
-    a->sec[q] = {static_cast<char*>(s[q].ptr), s[q].esz, s[q].per_env, s[q].place, s[q].clk, off};
+    a->sec[q] = {static_cast<char*>(*s[q].slot), s[q].esz, s[q].per_env, s[q].place, s[q].clk, off};
     if (s[q].clk == kClkSwst) a->swst_off = off;
     off += row_words(s[q]);
   }
@@ -1660,7 +1653,7 @@ static void record_args(gemb200_handle* h, RecArgs* a) {
   a->kstep = (uint32_t)h->n_steps;
   a->ring = a->dead > 0 ? (int)(h->n_steps % (uint64_t)a->dead) : 0;
   a->clock_dev = h->dev_clock ? h->d_clock : nullptr;
-  a->rngid = h->pf.rngid ? h->d_rngid : nullptr;
+  a->rngid = h->ids_in_use ? h->d_rngid : nullptr;
   a->seed_lo = (uint32_t)h->cfg.seed; a->seed_hi = (uint32_t)(h->cfg.seed >> 32);
   a->env_offset = h->cfg.env_index_offset;
 }
@@ -1683,7 +1676,7 @@ int gemb200_query_env_record(const gemb200_config* cfg, int32_t* words, uint64_t
 
 int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
-  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
   if (m < 0) return fail(GEMB200_E_INVALID, "m must be >= 0");
   if (m == 0) return GEMB200_OK;
   if (!rows) return fail(GEMB200_E_INVALID, "rows is NULL");
@@ -1702,7 +1695,7 @@ int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint
 int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
                         const int32_t* env_idx, int32_t m, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
-  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
   if (m < 0 || n_rows < 0) return fail(GEMB200_E_INVALID, "m and n_rows must be >= 0");
   RecArgs a;
   record_args(h, &a);
@@ -1794,7 +1787,7 @@ int gemb200_pack_rng_ids(gemb200_handle* h, const int32_t* env_idx, int32_t m, u
   if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
   DeviceGuard guard(h->cfg.device);
   const int64_t words = (int64_t)m * kRngIdWords;
-  pack_rng_ids_kernel<<<(unsigned)((words + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->pf.rngid ? h->d_rngid : nullptr, h->cfg.n_envs, (uint32_t)h->cfg.seed,
+  pack_rng_ids_kernel<<<(unsigned)((words + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->ids_in_use ? h->d_rngid : nullptr, h->cfg.n_envs, (uint32_t)h->cfg.seed,
                                                                                         (uint32_t)(h->cfg.seed >> 32), h->cfg.env_index_offset, id_clock_args(h), env_idx, m, ids);
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
@@ -1805,27 +1798,27 @@ int gemb200_adopt_rng_ids(gemb200_handle* h, const uint32_t* ids, int32_t n_ids,
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (h->cfg.layout != GEMB200_LAYOUT_AOS)
     return fail(GEMB200_E_INVALID, "adopted RNG identities are read by the per-env parameter instantiations, which need the row-per-env (AoS) I/O layout (DESIGN §7)");
-  if (h->n_draw > 0) return fail(GEMB200_E_INVALID, "RNG identities cannot be adopted while parameters are drawn per reset: snapshots are refused then (DESIGN §7)");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "RNG identities cannot be adopted while parameters are drawn per reset: snapshots are refused then (DESIGN §7)");
   if (m < 0 || n_ids < 0) return fail(GEMB200_E_INVALID, "m and n_ids must be >= 0");
   if (m == 0 || n_ids == 0) return GEMB200_OK;
   if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
   DeviceGuard guard(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (!h->pf.envp) {  // first adoption: the shared parameters into per-env blocks, so that the handle runs the ENVP instantiations (synchronises)
+  if (h->blocks == kBlocksNone) {  // first adoption: the shared parameters into per-env blocks, so that the handle runs the ENVP instantiations (synchronises)
     const int rc = fill_shared_blocks(h);
     if (rc) return rc;
-    h->pf.coef_shared = h->pd.coef_shared = 1;
+    h->blocks = kBlocksShared;
   }
   if (!h->d_rngid) CUDA_TRY(cudaMalloc(&h->d_rngid, (size_t)kRngIdWords * (size_t)h->cfg.n_envs * sizeof(uint32_t)));
-  if (!h->pf.rngid) {  // every other env keeps its own identity
+  if (!h->ids_in_use) {  // every other env keeps its own identity
     const int rc = launch_own_rng_ids(h, st);
     if (rc) return rc;
-    h->pf.rngid = h->pd.rngid = h->d_rngid;
+    h->ids_in_use = true;
   }
+  apply_mode(h);
   adopt_rng_ids_kernel<<<(m + 255) / 256, 256, 0, st>>>(h->d_rngid, h->cfg.n_envs, id_clock_args(h), ids, n_ids, row_idx, env_idx, m);
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
-  h->ids_adopted = true;
   return GEMB200_OK;
 }
 
