@@ -245,8 +245,13 @@ class ElectricMotorEnvironment(_EnvBase):
             return (state.double().cpu().numpy()[0], ref.double().cpu().numpy()[0]), {}
         return (state, ref), {}
 
-    def step(self, action):
-        """core.py:328-371"""
+    def step(self, action, reference=None):
+        """core.py:328-371.  reference (batched mode only): this step's reference feed, [N, n_ref] (SoA: [n_ref, N]) in the env's dtype on
+        its device.  It overwrites the stored value of EVERY reference slot before the step, exactly like `set_reference(reference)` before
+        `step(action)`, but in the step's own launch: no host synchronisation, so a captured closed loop (`capture_steps(...,
+        references=...)`) can track a caller-given reference.  Wrong shape, dtype or device: ValueError."""
+        if reference is not None and self._scalar:
+            raise TypeError("step(action, reference=...) needs a batched environment (num_envs=...); a scalar env takes set_reference()")
         sim = self._ensure_sim()
         if self._scalar:
             assert not self._terminated, "A reset is required before the environment can perform further steps"
@@ -258,7 +263,7 @@ class ElectricMotorEnvironment(_EnvBase):
             action = np.asarray(action).reshape(1, -1)
         if self._callbacks:
             self._call_callbacks("on_step_begin", self._physical_system.k, action)
-        obs, ref, reward, terminated = sim.step(action)
+        obs, ref, reward, terminated = sim.step(action) if reference is None else sim.step(action, reference)
         self._physical_system._k += 1
         state = obs if self._filter_identity else self._filter(obs)
         if self._callbacks:
@@ -269,15 +274,21 @@ class ElectricMotorEnvironment(_EnvBase):
             return (state.double().cpu().numpy()[0], ref.double().cpu().numpy()[0]), float(reward[0].item()), term, self._truncated, {}
         return (state, ref), reward, terminated.view(torch.bool), self._truncated, {}  # uint8 0/1 reinterpreted, no kernel
 
-    def rollout(self, actions, record_every=1):
+    def rollout(self, actions, record_every=1, references=None):
         """K consecutive `step` calls with pre-computed actions [K, N, n_act] in ONE kernel launch (open loop; bit-identical to calling
         `step` K times, core.py:328-371).  Returns ((states, references), rewards, terminateds) with a leading axis of K // record_every
         recorded steps (record_every = 0: only the last step, without the leading axis).  Batched mode only; callbacks see no
-        per-step hooks."""
+        per-step hooks.
+        references: a reference feed [K, N, n_ref] (SoA: [K, n_ref, N]) in the env's dtype on its device — a drive cycle, a test profile,
+        a recorded trajectory or the known future reference of an MPC horizon.  Step k first overwrites the stored value of EVERY reference
+        slot (not only the ExternalReferenceGenerator ones) with references[k]: the result is exactly that of K iterations of
+        `set_reference(references[k]); step(actions[k])`.  The returned reference of step k is what that loop returns: for an External
+        slot the value step k was scored against (the reset value on an env that was auto-reset in step k).  A policy that needs a preview
+        reads it from `references` itself.  Wrong shape, dtype, device or K: ValueError."""
         if self._scalar:
             raise TypeError("rollout() needs a batched environment (num_envs=...)")
         sim = self._ensure_sim()
-        obs, ref, reward, terminated = sim.rollout(actions, record_every)
+        obs, ref, reward, terminated = sim.rollout(actions, record_every) if references is None else sim.rollout(actions, record_every, references)
         k = int(actions.shape[0]) if hasattr(actions, "shape") else len(actions)
         self._physical_system._k += k
         if not self._filter_identity:
@@ -287,12 +298,14 @@ class ElectricMotorEnvironment(_EnvBase):
             obs = obs.index_select(dim, self._filter_index)
         return (obs, ref), reward, terminated.view(torch.bool)
 
-    def capture_steps(self, policy, n_steps, record=False, warmup=1):
+    def capture_steps(self, policy, n_steps, record=False, warmup=1, references=None):
         """`n_steps` closed-loop steps — action = policy(state, reference); env.step(action) — captured ONCE in a CUDA graph (graph.py);
-        `.replay()` of the returned object runs them with a single call.  Batched mode only."""
+        `.replay()` of the returned object runs them with a single call.  Batched mode only.  references: a static reference feed
+        [n_steps, N, n_ref] (SoA: [n_steps, n_ref, N]); step k of every replay is `step(action, reference=references[k])`, so refilling
+        the tensor in place between replays makes the next replay track the new values."""
         from .graph import CapturedSteps
 
-        return CapturedSteps(self, policy, n_steps, record=record, warmup=warmup)
+        return CapturedSteps(self, policy, n_steps, record=record, warmup=warmup, references=references)
 
     _MP_SLOT = dict(p=K.MP_P, r_s=K.MP_R_S, l_d=K.MP_L_D, l_q=K.MP_L_Q, psi_p=K.MP_PSI_P, j_rotor=K.MP_J_ROTOR, r_a=K.MP_R_A, l_a=K.MP_L_A, psi_e=K.MP_PSI_E,
                     r_e=K.MP_R_E, l_e=K.MP_L_E, l_e_prime=K.MP_L_E_PRIME, l_m=K.MP_L_M, k=K.MP_K, l_sigs=K.MP_L_SIGS, l_sigr=K.MP_L_SIGR, r_r=K.MP_R_E)

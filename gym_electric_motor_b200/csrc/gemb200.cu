@@ -701,8 +701,9 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
 // One launch over envs [begin, end) (end < 0: all).  new_call: this launch starts a new API call (fresh RNG call ids);
 // the chunks of one pipelined host step share them.  roll > 0: `roll` fused steps (rollout_kernel) whose call ids, step clock and
 // dead-time ring positions are exactly those of `roll` consecutive single-step calls; outputs every `every` steps (0: last only).
+// feed: the reference values of every step (StepParams::ref_feed), or NULL.
 static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, void* rew, uint8_t* term, cudaStream_t st,
-                   int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0) {
+                   int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
@@ -718,6 +719,7 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     p.gstep_lo = (uint32_t)g0; p.gstep_hi = (uint32_t)(g0 >> 32); p.clock_dev = dev_clock ? h->d_clock : nullptr;
     p.roll_steps = roll; p.record_every = every;
     p.action = action; p.obs = (real*)obs; p.ref_out = (real*)ref; p.reward = (real*)rew; p.term = term;
+    p.ref_feed = static_cast<const real*>(feed);
     set_roll_strides(h, p);
     return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
   });
@@ -920,11 +922,17 @@ int gemb200_step(gemb200_handle* h, const void* action, void* obs_out, void* ref
 
 int gemb200_rollout_record(gemb200_handle* h, const void* actions, int32_t n_steps, int32_t record_every, void* obs_out, void* ref_out,
                            void* reward_out, uint8_t* terminated_out, void* stream) {
+  return gemb200_rollout_record_ref(h, actions, nullptr, n_steps, record_every, obs_out, ref_out, reward_out, terminated_out, stream);
+}
+
+int gemb200_rollout_record_ref(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t record_every,
+                               void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
   if (record_every < 0 || record_every > n_steps) return fail(GEMB200_E_INVALID, "record_every must be in [0, n_steps]");
+  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
   DeviceGuard guard(h->cfg.device);
-  return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, record_every);
+  return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, record_every, references);
 }
 
 int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, void* obs_out, void* ref_out, void* reward_out,

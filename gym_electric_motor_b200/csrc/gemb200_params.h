@@ -261,6 +261,10 @@ struct StepParams {
   //      nullptr: every env draws with its own identity (seed, env_offset + i, 0, 0) ----
   const uint32_t* rngid;
   int32_t coef_shared;     // 1: the per-env blocks hold the shared parameters (made by the first adoption): reset observations from reset_obs
+  // ---- reference feed (gemb200_rollout_record_ref; read by the general and ENVP instantiations only, never PLAIN): the caller's reference
+  //      values of every step of this launch, [K][N][n_ref] (row-per-env) or [K][n_ref][N] (field-major).  Step k first overwrites the
+  //      stored value of EVERY slot with row k, as gemb200_set_reference would.  nullptr: no feed ----
+  const real* ref_feed;
 };
 constexpr int kRngIdWords = 8;
 

@@ -18,14 +18,20 @@ class CapturedSteps:
     synchronisation.  The first call sees `state0`, `reference0` (default: the env's current observation buffers, i.e. what the last
     reset / step returned).  After every `replay()` the attributes `state`, `reference`, `reward`, `terminated` hold the outputs of the
     last step (static tensors, overwritten by the next replay); with record=True `states`, `references`, `rewards`, `terminateds`
-    hold all `n_steps` of them.  Bit-identical to running the same loop eagerly."""
+    hold all `n_steps` of them.  Bit-identical to running the same loop eagerly.
 
-    def __init__(self, env, policy, n_steps, record=False, warmup=1):
+    references: a static reference feed [n_steps, N, n_ref] (SoA: [n_steps, n_ref, N]) in the env's dtype on its device.  Step k of every
+    replay runs `env.step(action, reference=references[k])`, reading row k where the tensor stands at replay time: refill it in place
+    between replays (never reallocate it) to track a new reference."""
+
+    def __init__(self, env, policy, n_steps, record=False, warmup=1, references=None):
         if getattr(env, "_scalar", True):
             raise TypeError("CapturedSteps needs a batched environment (num_envs=...)")
         self.env, self.n_steps = env, int(n_steps)
         sim = env._ensure_sim()
         self._sim = sim
+        self.reference_feed = None if references is None else sim._as_feed(references, self.n_steps)
+        feed = (lambda k: None) if references is None else (lambda k: self.reference_feed[k])
         dev = sim.device
         obs, ref, _, _ = sim._alloc_outputs()
         if warmup:  # lazy initialisation inside the policy (cuBLAS workspaces, autotuning) must not happen during capture; the warm-up steps
@@ -34,8 +40,8 @@ class CapturedSteps:
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(side):
-                for _ in range(int(warmup)):
-                    (st, rf), _, _, _, _ = env.step(policy(env._filter(obs), ref))
+                for j in range(int(warmup)):
+                    (st, rf), _, _, _, _ = env.step(policy(env._filter(obs), ref), feed(j % self.n_steps))
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
             sim.load_state_dict(sd)
@@ -48,8 +54,8 @@ class CapturedSteps:
         rec = [] if record else None
         with torch.cuda.graph(self.graph):
             st, rf = env._filter(obs), ref
-            for _ in range(self.n_steps):
-                (st, rf), rw, tm, _, _ = env.step(policy(st, rf))
+            for k in range(self.n_steps):
+                (st, rf), rw, tm, _, _ = env.step(policy(st, rf), feed(k))
                 if record:
                     rec.append((st.clone(), rf.clone(), rw.clone(), tm.clone()))
         env._physical_system._k -= self.n_steps  # capture ran the host side of env.step without executing anything

@@ -50,10 +50,11 @@ class GemVectorEnv:
         (state, ref), info = self.env.reset(seed=seed, options=options)
         return self._obs(state, ref), info
 
-    def step(self, actions):
+    def step(self, actions, reference=None):
+        """reference: this step's reference feed (ElectricMotorEnvironment.step), or None"""
         import torch
 
-        (state, ref), reward, terminated, truncated, info = self.env.step(actions)
+        (state, ref), reward, terminated, truncated, info = self.env.step(actions) if reference is None else self.env.step(actions, reference)
         truncations = torch.zeros_like(terminated)
         return self._obs(state, ref), reward, terminated, truncations, info
 

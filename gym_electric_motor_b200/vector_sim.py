@@ -172,9 +172,34 @@ class VectorSim:
             raise NotImplementedError(f"{what} is not available while parameters are drawn per reset: the drawn parameters are per-episode "
                                       "state that neither checkpoints nor snapshot rows carry (DESIGN.md §7); stop the draws first")
 
-    def step(self, action):
+    def _as_feed(self, references, k):
+        """check a reference feed of k steps: a contiguous device tensor of the handle's dtype, shaped [k, N, n_ref] (SoA: [k, n_ref, N]);
+        k = None: one step, [N, n_ref] (SoA: [n_ref, N]).  Nothing is converted: a feed is read in place by the launch (and by every replay
+        of a captured one)."""
+        if not self.n_ref:
+            raise ValueError("a reference feed needs reference slots: this configuration has n_ref == 0")
+        shape = self._shape(self.n_ref) if k is None else (int(k),) + self._shape(self.n_ref)
+        if not isinstance(references, torch.Tensor):
+            raise ValueError(f"references must be a {self.dtype} tensor of shape {shape} on {self.device}")
+        if references.dtype != self.dtype or references.device != self.device or tuple(references.shape) != shape:
+            raise ValueError(f"references must be {shape} {self.dtype} on {self.device}, got {tuple(references.shape)} {references.dtype} "
+                             f"on {references.device}")
+        if not references.is_contiguous():
+            raise ValueError("references must be contiguous")
+        return references
+
+    def step(self, action, reference=None):
         """env.step: returns (obs, ref_next, reward, terminated) device tensors (views of reused buffers unless
-        reuse_outputs=False)."""
+        reuse_outputs=False).  reference ([N, n_ref], SoA [n_ref, N], the handle's dtype, on the device): first overwrite the stored value
+        of every reference slot with it — `set_reference(reference); step(action)` in one stream-ordered, capturable launch (a K = 1
+        rollout with a reference feed)."""
+        if reference is not None:
+            r = self._as_feed(reference, None)
+            a = self._as_action(action)
+            obs, ref, rew, term = out = self._alloc_outputs()
+            K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(a), _ptr(r), 1, 0, _ptr(obs), _ptr(ref), _ptr(rew), _ptr(term),
+                                                         self._stream()), "gemb200_rollout_record_ref")
+            return out
         a = self._as_action(action)
         out = self._alloc_outputs()
         if self._reuse:
@@ -190,16 +215,20 @@ class VectorSim:
             K.check(rc, "gemb200_step")
         return out
 
-    def rollout(self, actions, record_every=0):
+    def rollout(self, actions, record_every=0, references=None):
         """K open-loop env.step calls fused into ONE launch (gemb200_rollout_record): every env's record stays in registers for all K
         steps; bit-identical to K calls of `step`.  actions: [K, N, n_act] (SoA layout: [K, n_act, N]).
         record_every = 0 -> the outputs of the last step (obs, ref, reward, terminated), shapes as `step`;
-        record_every = m >= 1 -> the outputs of steps m, 2m, ... stacked on a leading axis of length K // m (m = 1: full trajectory)."""
+        record_every = m >= 1 -> the outputs of steps m, 2m, ... stacked on a leading axis of length K // m (m = 1: full trajectory).
+        references ([K, N, n_ref], SoA [K, n_ref, N], the handle's dtype, on the device; gemb200_rollout_record_ref): step k first
+        overwrites the stored value of EVERY reference slot with references[k] — the same as K iterations of
+        `set_reference(references[k]); step(actions[k])`."""
         a = actions if (isinstance(actions, torch.Tensor) and actions.dtype == self.act_dtype and actions.device == self.device and actions.is_contiguous()) \
             else torch.as_tensor(actions, device=self.device).to(self.act_dtype).contiguous()
         k = int(a.shape[0])
         if a.numel() != k * self.n * self.n_act:
             raise ValueError(f"actions must hold K x {self.n} x {self.n_act} values")
+        r = None if references is None else self._as_feed(references, k)
         m = int(record_every)
         if m == 0:
             obs, ref, rew, term = self._alloc_outputs()
@@ -209,14 +238,24 @@ class VectorSim:
             ref = torch.empty((s,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device)
             rew = torch.empty((s, self.n), dtype=self.dtype, device=self.device)
             term = torch.empty((s, self.n), dtype=torch.uint8, device=self.device)
-        K.check(self._lib.gemb200_rollout_record(self._h, _ptr(a), k, m, _ptr(obs), _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term), self._stream()),
-                "gemb200_rollout_record")
+        if r is None:
+            K.check(self._lib.gemb200_rollout_record(self._h, _ptr(a), k, m, _ptr(obs), _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term),
+                                                     self._stream()), "gemb200_rollout_record")
+        else:
+            K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(a), _ptr(r), k, m, _ptr(obs), _ptr(ref), _ptr(rew), _ptr(term), self._stream()),
+                    "gemb200_rollout_record_ref")
         return obs, ref, rew, term
 
-    def rollout_into(self, actions, n_steps, record_every, obs, ref, rew, term):
-        """Raw variant for benchmarking: caller-owned output tensors (any may be None), no allocation, no conversion."""
-        K.check(self._lib.gemb200_rollout_record(self._h, _ptr(actions), int(n_steps), int(record_every), _ptr(obs), _ptr(ref) if self.n_ref else None,
-                                                 _ptr(rew), _ptr(term), self._stream()), "gemb200_rollout_record")
+    def rollout_into(self, actions, n_steps, record_every, obs, ref, rew, term, references=None):
+        """Raw variant for benchmarking: caller-owned output tensors (any may be None), no allocation, no conversion.  references: the
+        reference feed of `rollout`, checked like there."""
+        if references is None:
+            K.check(self._lib.gemb200_rollout_record(self._h, _ptr(actions), int(n_steps), int(record_every), _ptr(obs), _ptr(ref) if self.n_ref else None,
+                                                     _ptr(rew), _ptr(term), self._stream()), "gemb200_rollout_record")
+            return
+        r = self._as_feed(references, n_steps)
+        K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(actions), _ptr(r), int(n_steps), int(record_every), _ptr(obs), _ptr(ref),
+                                                     _ptr(rew), _ptr(term), self._stream()), "gemb200_rollout_record_ref")
 
     # ------------------------------------------------------------------ host-buffer API (numpy)
     def step_host(self, action, out=None):

@@ -311,6 +311,15 @@ int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, voi
 int gemb200_rollout_record(gemb200_handle* h, const void* actions, int32_t n_steps, int32_t record_every, void* obs_out, void* ref_out,
                            void* reward_out, uint8_t* terminated_out, void* stream);
 
+/* gemb200_rollout_record with a per-step reference feed: references[K][N][n_ref] (cfg->layout SoA: [K][n_ref][N]) in the handle's dtype,
+ * resident on the device.  Before step k, row k overwrites the stored value of EVERY reference slot, not only the External ones: the call
+ * gives exactly the outputs, final state and clock of K iterations of gemb200_set_reference(row k) + gemb200_step.  So the ref output of
+ * step k is what that sequence gives: for an External slot the value step k was scored against (the reset value on an env that was
+ * auto-reset in step k).  Stream-ordered, no host synchronisation; capturable in a CUDA graph under the device clock.  references ==
+ * NULL: exactly gemb200_rollout_record.  A feed into a configuration without reference slots (n_ref == 0) is GEMB200_E_INVALID. */
+int gemb200_rollout_record_ref(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t record_every,
+                               void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream);
+
 /* OdeSolver.y / set_initial_value (physical_systems/solvers.py:4-76): ODE state as double [N][n_ode]
  * (AoS, device), angle unwrapped to (-pi, pi].  Used for checkpointing and oracle injection. */
 int gemb200_get_ode_state(gemb200_handle* h, double* ode_out, void* stream);
