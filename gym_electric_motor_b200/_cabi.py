@@ -30,6 +30,7 @@ SUPPLY_IDEAL, SUPPLY_RC, SUPPLY_AC1 = 0, 1, 2
 DIST_UNIFORM, DIST_LOG_UNIFORM = 0, 1
 MAX_DRAW = MAX_MOTOR_PARAM + 8  # parameter slots of gemb200_set_param_randomization: motor slots, then load slots
 RNG_ID_WORDS = 8  # GEMB200_RNG_ID_WORDS: words of one RNG identity row (gemb200_pack_rng_ids)
+ENV_PARAM_SLOTS = MAX_DRAW  # GEMB200_ENV_PARAM_SLOTS: float64 slots of one parameter row (gemb200_pack_envs_params), the order of MAX_DRAW
 
 E_INVALID, E_CUDA, E_NOMEM, E_ABI = -1, -2, -3, -4
 
@@ -152,6 +153,7 @@ SYMBOLS = [
     "gemb200_peer_buffer_free", "gemb200_bind_peers", "gemb200_peer_signal", "gemb200_peer_wait", "gemb200_checkpoint_size", "gemb200_checkpoint_save", "gemb200_checkpoint_load", "gemb200_query_env_record",
     "gemb200_pack_envs", "gemb200_unpack_envs", "gemb200_set_param_randomization", "gemb200_get_env_params", "gemb200_launch_count",
     "gemb200_kernel_time_begin", "gemb200_kernel_time_end", "gemb200_pack_rng_ids", "gemb200_adopt_rng_ids", "gemb200_clear_rng_ids",
+    "gemb200_pack_envs_params", "gemb200_unpack_envs_params",
 ]
 
 
@@ -221,6 +223,8 @@ def load_library():
     lib.gemb200_pack_rng_ids.argtypes = [vp, vp, C.c_int32, vp, vp]
     lib.gemb200_adopt_rng_ids.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, vp]
     lib.gemb200_clear_rng_ids.argtypes = [vp, vp]
+    lib.gemb200_pack_envs_params.argtypes = [vp, vp, C.c_int32, vp, vp, vp]
+    lib.gemb200_unpack_envs_params.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_uint64, vp, vp, C.c_int32, vp]
     lib.gemb200_launch_count.argtypes = [vp]
     lib.gemb200_launch_count.restype = C.c_int64
     lib.gemb200_kernel_time_begin.argtypes = [vp, vp]

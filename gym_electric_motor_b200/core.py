@@ -345,7 +345,8 @@ class ElectricMotorEnvironment(_EnvBase):
         sequences, independent of sharding.  The call itself draws nothing (the usual pattern is this call, then `reset()`);
         `randomize_env_parameters()` without arguments stops drawing and the envs keep their last values.  Pole pairs cannot be drawn
         (ValueError); nor, for induction motors with random initial states, the parameters of their flux limits (NotImplementedError).
-        Needs the row-per-env (AoS) layout (ValueError).  While draws are on, checkpoints and snapshots are refused (DESIGN.md §7)."""
+        Needs the row-per-env (AoS) layout (ValueError).  While draws are on, checkpoints are refused, and so are snapshots and restores
+        unless they carry the parameters (`snapshot_envs(..., params=True)`, `restore_envs(..., params="source")`; DESIGN.md §7)."""
         if self._scalar:
             raise TypeError("randomize_env_parameters() needs a batched environment (num_envs=...)")
         from .randomization import encode_distributions
@@ -368,17 +369,23 @@ class ElectricMotorEnvironment(_EnvBase):
         vals = sim.env_params()
         return {name: vals[j] for j, name in enumerate(self._randomized_names)}
 
-    def snapshot_envs(self, idx=None, rng=False):
+    def snapshot_envs(self, idx=None, rng=False, params=False):
         """Branching support, the batched counterpart of `copy.deepcopy(env)`: the complete persistent state of envs `idx` (None: all;
         list, numpy array or tensor) as an `EnvSnapshot` of packed device rows, taken without a host synchronisation.  Host-side
         indices are range-checked (IndexError); a device index tensor is taken as given.  rng=True also takes the envs' RNG identities
-        (seed, global index and where their random streams stand), which `restore_envs(..., rng="source")` hands on.  Batched mode only."""
+        (seed, global index and where their random streams stand), which `restore_envs(..., rng="source")` hands on.  params=True also
+        takes their physical parameters (`snap.params`, float64 [m, 24] in the slot order of `_cabi.MP_*`, then `MAX_MOTOR_PARAM + LP_*`:
+        per-env values, drawn or set from the host, or the env's own), which `restore_envs(..., params="source")` hands on; it is allowed
+        while parameters are drawn per reset and needs the row-per-env layout (ValueError).  Batched mode only."""
         if self._scalar:
             raise TypeError("snapshot_envs() needs a batched environment (num_envs=...)")
-        from .snapshot import check_host_index
+        from .snapshot import check_host_index, check_params_layout
 
         sim = self._ensure_sim()
         idx = check_host_index(idx, sim.n, "idx")
+        if params:
+            check_params_layout(sim.soa)
+            return sim.snapshot(idx, rng=bool(rng), params=True)
         return sim.snapshot(idx, rng=True) if rng else sim.snapshot(idx)
 
     def clear_rng_identities(self):
@@ -389,7 +396,7 @@ class ElectricMotorEnvironment(_EnvBase):
             raise TypeError("clear_rng_identities() needs a batched environment (num_envs=...)")
         self._ensure_sim().clear_rng_ids()
 
-    def restore_envs(self, snapshot, idx=None, rows=None, rng="own"):
+    def restore_envs(self, snapshot, idx=None, rows=None, rng="own", params="own"):
         """Env idx[j] (None: env j) takes the state of snapshot row rows[j] (None: row j): physically the source env, continuing bit for
         bit except for the random numbers, which by default (rng="own") are the restored env's own from then on (its Wiener increments,
         periodic-generator parameters, switching choices, noise and later random resets).  `rows` fans one snapshot out to many envs without copying it.
@@ -399,17 +406,26 @@ class ElectricMotorEnvironment(_EnvBase):
         rng="source" (a snapshot taken with rng=True) gives `copy.deepcopy(env)` semantics instead: every restored env adopts its source's
         RNG identity and repeats the source's random numbers — same actions, same outputs, bit for bit, across terminations and resets.
         A later restore with rng="own", `clear_rng_identities()` or `reset(seed=...)` drops the identity.  It needs the row-per-env layout
-        (ValueError); while identities are adopted, `state_dict` / `load_state_dict` raise NotImplementedError (DESIGN.md §7)."""
+        (ValueError); while identities are adopted, `state_dict` / `load_state_dict` raise NotImplementedError (DESIGN.md §7).
+        params="source" (a snapshot taken with params=True) gives every restored env its row's physical parameters: it runs its current
+        episode on the source's plant, and with parameter draws on its next reset draws new values (with rng="source": the source's).  This
+        is what branching domain-randomised envs needs, and it is allowed while parameters are drawn per reset.  The values of
+        `snapshot.params` are used as given, so an edited copy restores an ensemble of plants; the pole-pair slot is ignored, and pole pairs
+        differing from this env's raise ValueError.  Afterwards the env runs per-env parameter blocks (DESIGN.md §7)."""
         if self._scalar:
             raise TypeError("restore_envs() needs a batched environment (num_envs=...)")
-        from .snapshot import check_host_index, check_layout, check_rng_mode
+        from .snapshot import check_host_index, check_layout, check_params_mode, check_rng_mode
 
         sim = self._ensure_sim()
         words, lid = sim.record_layout()
         check_layout(snapshot, words, lid)
         idx = check_host_index(idx, sim.n, "idx")
         rows = check_host_index(rows, len(snapshot), "rows")
-        if check_rng_mode(snapshot, rng, sim.soa):
+        take = check_params_mode(snapshot, params, sim.soa, sim.cfg.motor_param[K.MP_P])
+        adopt = check_rng_mode(snapshot, rng, sim.soa)
+        if take:
+            sim.restore(snapshot, idx, rows, rng="source" if adopt else "own", params="source")
+        elif adopt:
             sim.restore(snapshot, idx, rows, rng="source")
         else:
             sim.restore(snapshot, idx, rows)

@@ -1015,6 +1015,13 @@ __global__ void fill_env_params_kernel(real* envp, double* praw, const Coef<real
   envp[27 * nn + i] = k.inv_j; envp[28 * nn + i] = k.omega_lim; envp[29 * nn + i] = k.omega_lin;
   for (int s = 0; s < kMaxDraw; ++s) praw[s * nn + i] = raw.v[s];
 }
+// the configuration's physical parameters in the slot order of praw
+static RawParams config_params(const gemb200_handle* h) {
+  RawParams raw;
+  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
+  for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
+  return raw;
+}
 // no adopted identities any more: launches key every env by its own identity again, and blocks that only an adoption made go, so that the
 // handle runs its shared-coefficient kernels like a fresh one (the identity array stays allocated for the next adoption)
 static void drop_rng_ids(gemb200_handle* h) {
@@ -1027,9 +1034,7 @@ static int fill_shared_blocks(gemb200_handle* h) {
   const size_t nn = (size_t)h->cfg.n_envs;
   if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
   if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, (size_t)kMaxDraw * nn * sizeof(double)));
-  RawParams raw;
-  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
-  for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
+  const RawParams raw = config_params(h);
   const int grid = (int)((nn + 255) / 256);
   with_params(h, [&](auto& p) {
     using real = decltype(p.tau);
@@ -1671,20 +1676,8 @@ static int record_block(int stride) {  // largest block whose rows fit the defau
   return 0;
 }
 
-extern "C" {
-
-int gemb200_query_env_record(const gemb200_config* cfg, int32_t* words, uint64_t* layout_id) {
-  int rc = validate(cfg);
-  if (rc) return rc;
-  const int w = record_words(cfg);
-  if (words) *words = w;
-  if (layout_id) *layout_id = record_layout_id(cfg, w);
-  return GEMB200_OK;
-}
-
-int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream) {
-  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
-  if (draws_on(h)) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+// the state rows of gemb200_pack_envs / gemb200_unpack_envs, without their refusal under parameter draws
+static int pack_env_rows(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream) {
   if (m < 0) return fail(GEMB200_E_INVALID, "m must be >= 0");
   if (m == 0) return GEMB200_OK;
   if (!rows) return fail(GEMB200_E_INVALID, "rows is NULL");
@@ -1699,11 +1692,14 @@ int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint
   h->launches += 1;
   return GEMB200_OK;
 }
-
-int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
-                        const int32_t* env_idx, int32_t m, void* stream) {
-  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
-  if (draws_on(h)) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+// refuses rows of another record layout before anything else
+static int check_row_layout(gemb200_handle* h, uint64_t layout_id) {
+  if (layout_id != record_layout_id(&h->cfg, record_words(&h->cfg)))
+    return fail(GEMB200_E_INVALID, "unpack: the rows were packed from a handle with another record layout (motor, dtype, generators, dead time, ...)");
+  return GEMB200_OK;
+}
+static int unpack_env_rows(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
+                           const int32_t* env_idx, int32_t m, void* stream) {
   if (m < 0 || n_rows < 0) return fail(GEMB200_E_INVALID, "m and n_rows must be >= 0");
   RecArgs a;
   record_args(h, &a);
@@ -1719,6 +1715,30 @@ int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows,
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
   return GEMB200_OK;
+}
+
+extern "C" {
+
+int gemb200_query_env_record(const gemb200_config* cfg, int32_t* words, uint64_t* layout_id) {
+  int rc = validate(cfg);
+  if (rc) return rc;
+  const int w = record_words(cfg);
+  if (words) *words = w;
+  if (layout_id) *layout_id = record_layout_id(cfg, w);
+  return GEMB200_OK;
+}
+
+int gemb200_pack_envs(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  return pack_env_rows(h, env_idx, m, rows, stream);
+}
+
+int gemb200_unpack_envs(gemb200_handle* h, const uint32_t* rows, int32_t n_rows, uint64_t layout_id, const int32_t* row_idx,
+                        const int32_t* env_idx, int32_t m, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (draws_on(h)) return fail(GEMB200_E_INVALID, "snapshot rows do not carry the parameters drawn per reset; switch the draws off first (DESIGN §7)");
+  return unpack_env_rows(h, rows, n_rows, layout_id, row_idx, env_idx, m, stream);
 }
 
 }  // extern "C"
@@ -1786,6 +1806,31 @@ static int launch_own_rng_ids(gemb200_handle* h, cudaStream_t st) {
   return GEMB200_OK;
 }
 
+// gemb200_adopt_rng_ids without its refusals (layout, parameter draws)
+static int adopt_rng_id_rows(gemb200_handle* h, const uint32_t* ids, int32_t n_ids, const int32_t* row_idx, const int32_t* env_idx, int32_t m,
+                             cudaStream_t st) {
+  if (m < 0 || n_ids < 0) return fail(GEMB200_E_INVALID, "m and n_ids must be >= 0");
+  if (m == 0 || n_ids == 0) return GEMB200_OK;
+  if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
+  DeviceGuard guard(h->cfg.device);
+  if (h->blocks == kBlocksNone) {  // first adoption: the shared parameters into per-env blocks, so that the handle runs the ENVP instantiations (synchronises)
+    const int rc = fill_shared_blocks(h);
+    if (rc) return rc;
+    h->blocks = kBlocksShared;
+  }
+  if (!h->d_rngid) CUDA_TRY(cudaMalloc(&h->d_rngid, (size_t)kRngIdWords * (size_t)h->cfg.n_envs * sizeof(uint32_t)));
+  if (!h->ids_in_use) {  // every other env keeps its own identity
+    const int rc = launch_own_rng_ids(h, st);
+    if (rc) return rc;
+    h->ids_in_use = true;
+  }
+  apply_mode(h);
+  adopt_rng_ids_kernel<<<(m + 255) / 256, 256, 0, st>>>(h->d_rngid, h->cfg.n_envs, id_clock_args(h), ids, n_ids, row_idx, env_idx, m);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return GEMB200_OK;
+}
+
 extern "C" {
 
 int gemb200_pack_rng_ids(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* ids, void* stream) {
@@ -1807,27 +1852,7 @@ int gemb200_adopt_rng_ids(gemb200_handle* h, const uint32_t* ids, int32_t n_ids,
   if (h->cfg.layout != GEMB200_LAYOUT_AOS)
     return fail(GEMB200_E_INVALID, "adopted RNG identities are read by the per-env parameter instantiations, which need the row-per-env (AoS) I/O layout (DESIGN §7)");
   if (draws_on(h)) return fail(GEMB200_E_INVALID, "RNG identities cannot be adopted while parameters are drawn per reset: snapshots are refused then (DESIGN §7)");
-  if (m < 0 || n_ids < 0) return fail(GEMB200_E_INVALID, "m and n_ids must be >= 0");
-  if (m == 0 || n_ids == 0) return GEMB200_OK;
-  if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
-  DeviceGuard guard(h->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (h->blocks == kBlocksNone) {  // first adoption: the shared parameters into per-env blocks, so that the handle runs the ENVP instantiations (synchronises)
-    const int rc = fill_shared_blocks(h);
-    if (rc) return rc;
-    h->blocks = kBlocksShared;
-  }
-  if (!h->d_rngid) CUDA_TRY(cudaMalloc(&h->d_rngid, (size_t)kRngIdWords * (size_t)h->cfg.n_envs * sizeof(uint32_t)));
-  if (!h->ids_in_use) {  // every other env keeps its own identity
-    const int rc = launch_own_rng_ids(h, st);
-    if (rc) return rc;
-    h->ids_in_use = true;
-  }
-  apply_mode(h);
-  adopt_rng_ids_kernel<<<(m + 255) / 256, 256, 0, st>>>(h->d_rngid, h->cfg.n_envs, id_clock_args(h), ids, n_ids, row_idx, env_idx, m);
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 1;
-  return GEMB200_OK;
+  return adopt_rng_id_rows(h, ids, n_ids, row_idx, env_idx, m, (cudaStream_t)stream);
 }
 
 int gemb200_clear_rng_ids(gemb200_handle* h, void* stream) {
@@ -1835,6 +1860,145 @@ int gemb200_clear_rng_ids(gemb200_handle* h, void* stream) {
   (void)stream;  // launches enqueued before the call keep the identities they were launched with
   drop_rng_ids(h);
   return GEMB200_OK;
+}
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------------------------
+// Per-env physical parameters in snapshots (gemb200_pack_envs_params / gemb200_unpack_envs_params; row format in include/gemb200.h)
+// ----------------------------------------------------------------------------------------------------------------
+// A parameter row is the env's praw column: kMaxDraw doubles.  Both kernels stage a block's rows in shared memory like pack_envs_kernel /
+// unpack_envs_kernel: the planar praw[kMaxDraw][n] is read and written with consecutive threads on consecutive envs, the [m][kMaxDraw]
+// rows word-contiguously by the whole block.
+static_assert(kMaxDraw == GEMB200_ENV_PARAM_SLOTS, "parameter row width");
+constexpr int kParBlock = 128;
+constexpr int kParStride = kMaxDraw + 1;  // odd stride in doubles: a half-warp's 8-byte shared accesses to its rows hit distinct banks
+
+// rows[j] = parameters of env env_idx[j] (NULL: j); praw NULL (a handle without per-env blocks): the configuration's, from `cfg`
+__global__ void __launch_bounds__(kParBlock) pack_env_params_kernel(const double* __restrict__ praw, const RawParams cfg, int n,
+                                                                    const int32_t* __restrict__ env_idx, int m, double* __restrict__ rows) {
+  __shared__ double srow[kParBlock * kParStride];
+  __shared__ int ok[kParBlock];
+  const int t = threadIdx.x, j0 = blockIdx.x * kParBlock, j = j0 + t;
+  bool valid = false;
+  if (j < m) {
+    const int i = env_idx ? env_idx[j] : j;
+    valid = i >= 0 && i < n;
+    if (valid) {
+      double* row = srow + t * kParStride;
+      if (praw) {
+        for (int s = 0; s < kMaxDraw; ++s) row[s] = praw[(size_t)s * n + i];
+      } else {
+        for (int s = 0; s < kMaxDraw; ++s) row[s] = cfg.v[s];
+      }
+    }
+  }
+  ok[t] = valid;
+  __syncthreads();
+  const int total = min(kParBlock, m - j0) * kMaxDraw;
+  double* dst = rows + (size_t)j0 * kMaxDraw;
+  for (int k = t; k < total; k += kParBlock) {
+    const int e = k / kMaxDraw, w = k - e * kMaxDraw;
+    if (ok[e]) dst[k] = srow[e * kParStride + w];
+  }
+}
+
+// Env i's column of the per-env parameter block envp [kCoefWords][n], derived from its physical parameters prm[kMaxDraw] by derive_coef
+// (gemb200_model.h), the derivation of the parameter draws and of gemb200_set_env_params.  The same stores end redraw_env_params
+// (gemb200_kernels.cuh); calling this function from there changes the register allocation of every reset kernel and ENVP step / rollout
+// kernel of the step translation units (DESIGN §4), so the eight lines are kept in both places.
+template <typename real>
+__device__ __forceinline__ void write_env_coef(int motor_kind, const double* prm, real* envp, unsigned i, size_t n) {
+  ModelCoef mc;
+  derive_coef(motor_kind, prm, prm + GEMB200_MAX_MOTOR_PARAM, &mc);
+  real* e = envp + i;
+  for (int w = 0; w < 20; ++w) e[(size_t)w * n] = (real)mc.c[w];
+  for (int w = 0; w < 4; ++w) e[(size_t)(20 + w) * n] = (real)mc.tq[w];
+  e[(size_t)24 * n] = (real)prm[GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_A];
+  e[(size_t)25 * n] = (real)prm[GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_B];
+  e[(size_t)26 * n] = (real)prm[GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_C];
+  e[(size_t)27 * n] = (real)mc.inv_j; e[(size_t)28 * n] = (real)mc.omega_lim; e[(size_t)29 * n] = (real)mc.omega_lin;
+}
+
+// env env_idx[j] (NULL: j) takes parameter row row_idx[j] (NULL: j): every slot but the pole pairs (per handle: the angle increments are
+// prepared on the host) into praw, and the coefficients derived from them into its envp column (write_env_coef, as a parameter draw does)
+template <typename real>
+__global__ void __launch_bounds__(kParBlock) adopt_env_params_kernel(double* __restrict__ praw, real* __restrict__ envp, int n, int motor_kind,
+                                                                     const double* __restrict__ rows, int n_rows, const int32_t* __restrict__ row_idx,
+                                                                     const int32_t* __restrict__ env_idx, int m) {
+  __shared__ double srow[kParBlock * kParStride];
+  __shared__ int src[kParBlock];
+  const int t = threadIdx.x, j0 = blockIdx.x * kParBlock, j = j0 + t;
+  int i = -1, r = -1;
+  if (j < m) {
+    r = row_idx ? row_idx[j] : j;
+    i = env_idx ? env_idx[j] : j;
+    if (r < 0 || r >= n_rows || i < 0 || i >= n) r = -1;
+  }
+  src[t] = r;
+  __syncthreads();
+  const int total = min(kParBlock, m - j0) * kMaxDraw;
+  for (int k = t; k < total; k += kParBlock) {
+    const int e = k / kMaxDraw, w = k - e * kMaxDraw;
+    const int rr = src[e];
+    if (rr >= 0) srow[e * kParStride + w] = __ldg(rows + (size_t)rr * kMaxDraw + w);
+  }
+  __syncthreads();
+  if (r < 0) return;
+  const size_t nn = (size_t)n;
+  const double* row = srow + t * kParStride;
+  double prm[kMaxDraw];
+#pragma unroll
+  for (int s = 0; s < kMaxDraw; ++s) prm[s] = row[s];
+  prm[GEMB200_MP_P] = praw[(size_t)GEMB200_MP_P * nn + i];
+#pragma unroll
+  for (int s = 0; s < kMaxDraw; ++s)
+    if (s != GEMB200_MP_P) praw[(size_t)s * nn + i] = prm[s];
+  write_env_coef<real>(motor_kind, prm, envp, (unsigned)i, nn);
+}
+
+extern "C" {
+
+int gemb200_pack_envs_params(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, double* params, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (h->cfg.layout != GEMB200_LAYOUT_AOS) return fail(GEMB200_E_INVALID, "parameter rows need the row-per-env (AoS) I/O layout (per-env parameter blocks)");
+  if (!rows || !params) return fail(GEMB200_E_INVALID, "rows and params are required");
+  const int rc = pack_env_rows(h, env_idx, m, rows, stream);
+  if (rc || m == 0) return rc;
+  DeviceGuard guard(h->cfg.device);
+  pack_env_params_kernel<<<(m + kParBlock - 1) / kParBlock, kParBlock, 0, (cudaStream_t)stream>>>(
+      h->blocks != kBlocksNone ? h->d_praw : nullptr, config_params(h), h->cfg.n_envs, env_idx, m, params);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return GEMB200_OK;
+}
+
+int gemb200_unpack_envs_params(gemb200_handle* h, const uint32_t* rows, const double* params, const uint32_t* ids, int32_t n_rows,
+                               uint64_t layout_id, const int32_t* row_idx, const int32_t* env_idx, int32_t m, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (h->cfg.layout != GEMB200_LAYOUT_AOS) return fail(GEMB200_E_INVALID, "parameter rows need the row-per-env (AoS) I/O layout (per-env parameter blocks)");
+  if (!rows || !params) return fail(GEMB200_E_INVALID, "rows and params are required");
+  if (m < 0 || n_rows < 0) return fail(GEMB200_E_INVALID, "m and n_rows must be >= 0");
+  int rc = check_row_layout(h, layout_id);
+  if (rc || m == 0 || n_rows == 0) return rc;
+  DeviceGuard guard(h->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h->blocks == kBlocksNone) {  // no per-env blocks yet: every other env keeps the shared parameters (synchronises)
+    rc = fill_shared_blocks(h);
+    if (rc) return rc;
+  }
+  h->blocks = kBlocksCaller;  // the blocks hold rows of the caller's now
+  apply_mode(h);
+  rc = unpack_env_rows(h, rows, n_rows, layout_id, row_idx, env_idx, m, stream);
+  if (rc) return rc;
+  with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    adopt_env_params_kernel<real><<<(m + kParBlock - 1) / kParBlock, kParBlock, 0, st>>>(h->d_praw, static_cast<real*>(h->d_envp), h->cfg.n_envs,
+                                                                                          h->cfg.motor_kind, params, n_rows, row_idx, env_idx, m);
+  });
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  return ids ? adopt_rng_id_rows(h, ids, n_rows, row_idx, env_idx, m, st) : GEMB200_OK;
 }
 
 }  // extern "C"

@@ -6,29 +6,41 @@ plain device `torch.int32` tensor [m, words] that the caller may keep, concatena
 another batch size, seed or index offset, or with other per-env parameters.  A restored env continues exactly like its source, except
 that it draws the random numbers of its own (seed, global env index) from then on — unless the snapshot was taken with `rng=True` and is
 restored with `rng="source"`: the env then adopts its source's RNG identity and repeats the source's draws (copy.deepcopy semantics).
+A snapshot taken with `params=True` also holds the envs' physical parameters; restored with `params="source"`, every env takes its source's
+(its own per-env values, drawn or set from the host) and runs its current episode on the source's plant.
 """
 import numpy as np
 import torch
 
-from ._cabi import RNG_ID_WORDS
+from ._cabi import ENV_PARAM_SLOTS, MP_P, RNG_ID_WORDS
 
 
 class EnvSnapshot:
     """Packed state of m envs: `rows` [m, words] int32 on the device, `layout_id` of the record layout, `dtype` of the handle's state,
-    `rng` [m, RNG_ID_WORDS] int32 = the envs' RNG identities (gemb200_pack_rng_ids) or None.
+    `rng` [m, RNG_ID_WORDS] int32 = the envs' RNG identities (gemb200_pack_rng_ids) or None,
+    `params` [m, ENV_PARAM_SLOTS] float64 = the envs' physical parameters (gemb200_pack_envs_params; slots `_cabi.MP_*`, then
+    `_cabi.MAX_MOTOR_PARAM + _cabi.LP_*`) or None, and `pole_pairs`, the source handle's pole pairs (host float) when `params` is set.
+    `params` is a plain tensor: editing it before a restore gives the restored envs the edited values (an ensemble of plants).
     `len(snap)` is m; `snap[k]`, `snap[a:b]`, `snap[index list / tensor]` are sub-snapshots of the selected rows."""
 
-    __slots__ = ("rows", "layout_id", "dtype", "rng")
+    __slots__ = ("rows", "layout_id", "dtype", "rng", "params", "pole_pairs")
 
-    def __init__(self, rows, layout_id, dtype, rng=None):
+    def __init__(self, rows, layout_id, dtype, rng=None, params=None, pole_pairs=None):
         if not isinstance(rows, torch.Tensor) or rows.dtype != torch.int32 or rows.dim() != 2:
             raise ValueError("EnvSnapshot rows must be a 2-D torch.int32 tensor [m, words]")
         if rng is not None and (not isinstance(rng, torch.Tensor) or rng.dtype != torch.int32 or tuple(rng.shape) != (rows.shape[0], RNG_ID_WORDS)):
             raise ValueError(f"EnvSnapshot rng must be a torch.int32 tensor [m, {RNG_ID_WORDS}] with one row per snapshot row")
+        if params is not None:
+            if not isinstance(params, torch.Tensor) or params.dtype != torch.float64 or tuple(params.shape) != (rows.shape[0], ENV_PARAM_SLOTS):
+                raise ValueError(f"EnvSnapshot params must be a torch.float64 tensor [m, {ENV_PARAM_SLOTS}] with one row per snapshot row")
+            if pole_pairs is None:
+                raise ValueError("EnvSnapshot params need the source's pole_pairs")
         self.rows = rows
         self.layout_id = int(layout_id)
         self.dtype = dtype
         self.rng = rng
+        self.params = params
+        self.pole_pairs = None if params is None else float(pole_pairs)
 
     def __len__(self):
         return int(self.rows.shape[0])
@@ -47,12 +59,15 @@ class EnvSnapshot:
             sel = idx
         else:
             sel = torch.as_tensor(np.asarray(idx) if not isinstance(idx, torch.Tensor) else idx, device=self.rows.device).long()
-        rng = None if self.rng is None else self.rng[sel if isinstance(sel, slice) else sel.to(self.rng.device)].contiguous()
-        return EnvSnapshot(self.rows[sel].contiguous(), self.layout_id, self.dtype, rng)
+
+        def pick(t):
+            return None if t is None else t[sel if isinstance(sel, slice) else sel.to(t.device)].contiguous()
+
+        return EnvSnapshot(self.rows[sel].contiguous(), self.layout_id, self.dtype, pick(self.rng), pick(self.params), self.pole_pairs)
 
     def __repr__(self):
         return (f"EnvSnapshot(m={len(self)}, words={self.words}, layout_id={self.layout_id:#018x}, dtype={self.dtype}, "
-                f"rng={'yes' if self.rng is not None else 'no'})")
+                f"rng={'yes' if self.rng is not None else 'no'}, params={'yes' if self.params is not None else 'no'})")
 
 
 def check_host_index(idx, bound, what):
@@ -79,6 +94,28 @@ def check_rng_mode(snap, rng, soa):
         if soa:
             raise ValueError("adopted RNG identities need the row-per-env layout (layout='aos'), like per-env parameter blocks (DESIGN.md §7)")
     return rng == "source"
+
+
+def check_params_layout(soa):
+    """ValueError on the field-major layout: parameter rows belong to per-env parameter blocks, which need the row-per-env layout"""
+    if soa:
+        raise ValueError("parameter rows need the row-per-env layout (layout='aos'), like every per-env parameter block (DESIGN.md §7)")
+
+
+def check_params_mode(snap, params, soa, pole_pairs):
+    """the `params` argument of a restore: "own" (the envs keep their physical parameters) or "source" (they take the snapshot's, which
+    needs a snapshot taken with params=True, the row-per-env layout and the source's pole pairs, which are per handle); ValueError
+    otherwise"""
+    if params not in ("own", "source"):
+        raise ValueError(f"params must be 'own' or 'source', got {params!r}")
+    if params == "source":
+        if snap.params is None:
+            raise ValueError("params='source' needs a snapshot taken with params=True (it carries no physical parameters)")
+        check_params_layout(soa)
+        if float(snap.pole_pairs) != float(pole_pairs):
+            raise ValueError(f"params='source': the snapshot's pole pairs ({snap.pole_pairs:g}) differ from this env's ({float(pole_pairs):g}); "
+                             "pole pairs are per env kind, not per env")
+    return params == "source"
 
 
 def check_layout(snap, words, layout_id):

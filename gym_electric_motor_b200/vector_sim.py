@@ -337,37 +337,50 @@ class VectorSim:
         t = idx if isinstance(idx, torch.Tensor) else torch.as_tensor(np.asarray(idx, dtype=np.int64).reshape(-1))
         return t.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
 
-    def snapshot(self, idx=None, rng=False):
+    def snapshot(self, idx=None, rng=False, params=False):
         """Pack the persistent state of envs `idx` (None: all) into an EnvSnapshot (gemb200_pack_envs; stream-ordered, no host sync).
         Row j holds env idx[j]; a device index entry out of range leaves its row uninitialised.  rng=True also packs the envs' effective
-        RNG identities (gemb200_pack_rng_ids) into `snap.rng`, for restore(..., rng="source")."""
-        from .snapshot import EnvSnapshot
+        RNG identities (gemb200_pack_rng_ids) into `snap.rng`, for restore(..., rng="source").  params=True also packs their physical
+        parameters (gemb200_pack_envs_params) into `snap.params`, for restore(..., params="source"); allowed while parameters are drawn."""
+        from .snapshot import EnvSnapshot, check_params_layout
 
-        self._refuse_while_drawing("snapshot")
+        if params:
+            check_params_layout(self.soa)
+        else:
+            self._refuse_while_drawing("snapshot")
         words, lid = self.record_layout()
         ii = self._dev_index(idx)
         m = self.n if ii is None else int(ii.numel())
         rows = torch.empty((m, words), dtype=torch.int32, device=self.device)
-        K.check(self._lib.gemb200_pack_envs(self._h, _ptr(ii), m, _ptr(rows), self._stream()), "gemb200_pack_envs")
+        prm = None
+        if params:
+            prm = torch.empty((m, K.ENV_PARAM_SLOTS), dtype=torch.float64, device=self.device)
+            K.check(self._lib.gemb200_pack_envs_params(self._h, _ptr(ii), m, _ptr(rows), _ptr(prm), self._stream()), "gemb200_pack_envs_params")
+        else:
+            K.check(self._lib.gemb200_pack_envs(self._h, _ptr(ii), m, _ptr(rows), self._stream()), "gemb200_pack_envs")
         ids = None
         if rng:
             ids = torch.empty((m, K.RNG_ID_WORDS), dtype=torch.int32, device=self.device)
             K.check(self._lib.gemb200_pack_rng_ids(self._h, _ptr(ii), m, _ptr(ids), self._stream()), "gemb200_pack_rng_ids")
-        return EnvSnapshot(rows, lid, self.dtype, ids)
+        return EnvSnapshot(rows, lid, self.dtype, ids, prm, float(self.cfg.motor_param[K.MP_P]) if params else None)
 
     def clear_rng_ids(self):
         """every env draws with its own RNG identity again (gemb200_clear_rng_ids; stream-ordered)"""
         K.check(self._lib.gemb200_clear_rng_ids(self._h, self._stream()), "gemb200_clear_rng_ids")
         self._ids_adopted = False
 
-    def restore(self, snap, idx=None, rows=None, rng="own"):
+    def restore(self, snap, idx=None, rows=None, rng="own", params="own"):
         """Env idx[j] (None: j) takes the state of snapshot row rows[j] (None: j) (gemb200_unpack_envs; stream-ordered, no host sync).
         `rows` fans one snapshot out: restore(snap, idx=range(C * m), rows=np.repeat(range(m), C)) copies every row into C envs.
         Device index entries out of range are skipped.  rng="own": the envs draw their own random numbers from then on; rng="source": they
-        adopt the snapshot's RNG identities (gemb200_adopt_rng_ids) and repeat their sources' draws."""
-        from .snapshot import check_layout, check_rng_mode
+        adopt the snapshot's RNG identities (gemb200_adopt_rng_ids) and repeat their sources' draws.  params="own": the envs keep their
+        physical parameters; params="source": they take the snapshot's (gemb200_unpack_envs_params, one call with the state and, with
+        rng="source", the identities), which is allowed while parameters are drawn per reset."""
+        from .snapshot import check_layout, check_params_mode, check_rng_mode
 
-        self._refuse_while_drawing("restore")
+        take = check_params_mode(snap, params, self.soa, self.cfg.motor_param[K.MP_P])
+        if not take:
+            self._refuse_while_drawing("restore")
         words, lid = self.record_layout()
         check_layout(snap, words, lid)
         adopt = check_rng_mode(snap, rng, self.soa)
@@ -375,9 +388,17 @@ class VectorSim:
         if ii is not None and rr is not None and ii.numel() != rr.numel():
             raise ValueError(f"idx ({ii.numel()}) and rows ({rr.numel()}) must have the same length")
         m = int(ii.numel()) if ii is not None else (int(rr.numel()) if rr is not None else min(len(snap), self.n))
-        if snap.rows.device != self.device or (adopt and snap.rng.device != self.device):
+        if snap.rows.device != self.device or (adopt and snap.rng.device != self.device) or (take and snap.params.device != self.device):
             raise ValueError(f"snapshot rows are on {snap.rows.device}, this handle on {self.device}: move the rows first")
         data = snap.rows.contiguous()
+        if take:
+            prm = snap.params.contiguous()
+            ids = snap.rng.contiguous() if adopt else None
+            K.check(self._lib.gemb200_unpack_envs_params(self._h, _ptr(data), _ptr(prm), _ptr(ids), len(snap), C.c_uint64(lid), _ptr(rr), _ptr(ii), m,
+                                                         self._stream()), "gemb200_unpack_envs_params")
+            if adopt:
+                self._ids_adopted = True
+            return
         K.check(self._lib.gemb200_unpack_envs(self._h, _ptr(data), len(snap), C.c_uint64(lid), _ptr(rr), _ptr(ii), m, self._stream()),
                 "gemb200_unpack_envs")
         if adopt:

@@ -369,7 +369,8 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
  * Refused (GEMB200_E_INVALID): pole pairs (host-prepared angle increments), the flux-limit parameters l_m, l_sigs, l_sigr, r_s, r_r of an
  * induction motor with random initial states (host-prepared init_im), the field-major (SoA) I/O layout, repeated or unknown slots and bad
  * bounds.  While draws are on, gemb200_checkpoint_save / _load and gemb200_pack_envs / _unpack_envs return GEMB200_E_INVALID: the drawn
- * parameters are per-episode state that neither format carries.  Synchronises the device. */
+ * parameters are per-episode state that neither format carries (gemb200_pack_envs_params / _unpack_envs_params below carry them with the
+ * state rows).  Synchronises the device. */
 enum gemb200_dist_kind { GEMB200_DIST_UNIFORM = 0, GEMB200_DIST_LOG_UNIFORM = 1 };
 int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t* slot, const int32_t* kind, const double* lo, const double* hi);
 /* Stream-ordered copy of the stored values of the drawn parameters into the device buffer out[n][n_envs] (handle dtype; order of the slots
@@ -426,7 +427,8 @@ int gemb200_checkpoint_load(gemb200_handle* h, const void* host_blob);
  * bit pattern in fp32, the integral double value in fp64): the sub-episode ends, the start step of a slot whose current generator is
  * periodic (sinus / step / sawtooth / triangular), and the super-episode ends.  Unpack re-bases them on the destination's step count.
  * Not in the row: the per-env parameter table (configuration, like in the checkpoint) and the RNG identity — a restored env draws the
- * random numbers of ITS OWN (seed, global index) from then on, unless it adopts its source's (gemb200_adopt_rng_ids below).
+ * random numbers of ITS OWN (seed, global index) from then on, unless it adopts its source's (gemb200_adopt_rng_ids below); and keeps
+ * its own physical parameters, unless it takes its source's (gemb200_unpack_envs_params below).
  * layout_id: FNV-1a over what decides the row format (dtype, motor, n_ode, n_ref, generator kinds and switched grouping, switching-state
  * array, dead time and its order and queue width, state-op kinds, supply, external speed load, induction motor with random initial
  * states); not over n_envs, seed, offsets, device, tau, solver, parameters, limits, reward, constraints, autoreset or layout. */
@@ -467,6 +469,31 @@ int gemb200_pack_rng_ids(gemb200_handle* h, const int32_t* env_idx, int32_t m, u
 int gemb200_adopt_rng_ids(gemb200_handle* h, const uint32_t* ids, int32_t n_ids, const int32_t* row_idx, const int32_t* env_idx, int32_t m, void* stream);
 /* every env draws with its own identity again */
 int gemb200_clear_rng_ids(gemb200_handle* h, void* stream);
+
+/* Per-env physical parameters in snapshots (opt-in; DESIGN §7): branch and deep-copy envs whose parameters are their own — set from the
+ * host (gemb200_set_env_params) or drawn at every reset (gemb200_set_param_randomization).  A parameter row is GEMB200_ENV_PARAM_SLOTS
+ * doubles in the slot order of gemb200_config: motor_param[GEMB200_MP_*], then load_param[GEMB200_LP_*] (the slot numbers of
+ * gemb200_set_param_randomization).
+ * gemb200_pack_envs_params is gemb200_pack_envs plus the parameter rows params[j][..] of env env_idx[j]: an env's per-env values, copied
+ * exactly (drawn values are stored rounded to the handle's dtype), or the configuration's on a handle without per-env blocks.
+ * gemb200_unpack_envs_params is gemb200_unpack_envs plus parameter adoption, plus identity adoption when ids is non-NULL (the
+ * gemb200_adopt_rng_ids semantics, ids[row_idx[j]] with the same n_rows): env env_idx[j] stores every slot of row row_idx[j] except the
+ * pole pairs, which are per handle (the angle increments are prepared on the host; the caller checks that source and destination agree),
+ * and its per-env coefficients are derived from them on the device by the code that derives drawn parameters.  The restored env then runs
+ * its current episode on its source's plant; with draws on, its next reset draws new values as usual (with an adopted identity: its
+ * source's draws).  Rows are used as given, like gemb200_set_env_params rows, but not checked: a zero inductance gives non-finite
+ * coefficients.  For an induction motor with random initial states the flux limits (init_im) stay the handle's, derived on the host from
+ * the configuration: a row with other l_m, l_sigs, l_sigr, r_s or r_r behaves like a gemb200_set_env_params row with those values.
+ * After an unpack with params the handle's per-env blocks are the caller's: its other envs keep their values (the shared parameters on a
+ * handle without blocks), but derive a constant initial state's reset observation on the device (DESIGN §4: last bits of the induction
+ * motors).  Both calls are accepted while parameters are drawn per reset, need the row-per-env I/O layout and non-NULL rows and params
+ * (GEMB200_E_INVALID otherwise), are stream-ordered and can be captured in a CUDA graph — except the first unpack on a handle without
+ * per-env blocks, which fills them from the shared parameters and synchronises the device.  gemb200_pack_envs / _unpack_envs, their row
+ * format and layout_id are unchanged, and still refused while draws are on. */
+#define GEMB200_ENV_PARAM_SLOTS 24 /* GEMB200_MAX_MOTOR_PARAM motor slots, then 8 load slots */
+int gemb200_pack_envs_params(gemb200_handle* h, const int32_t* env_idx, int32_t m, uint32_t* rows, double* params, void* stream);
+int gemb200_unpack_envs_params(gemb200_handle* h, const uint32_t* rows, const double* params, const uint32_t* ids, int32_t n_rows,
+                               uint64_t layout_id, const int32_t* row_idx, const int32_t* env_idx, int32_t m, void* stream);
 
 /* Introspection used by bench.py: number of kernel launches issued through this handle so far, and the
  * CUDA-event time in ms of the step launches since the last call (see DESIGN.md "Measurement"). */

@@ -1,6 +1,6 @@
 """Per-env snapshot throughput (gemb200_pack_envs / gemb200_unpack_envs) and a random-shooting MPC control step built on it.
 
-    python tools/branch_bench.py [--envs 1048576] [--reps 20] [--rng own|source]
+    python tools/branch_bench.py [--envs 1048576] [--reps 20] [--rng own|source] [--params]
 
 Prints the GPU name and power limit, then one JSON line per measurement (CUDA events, median over --reps):
   1. pack and unpack of all envs of Cont-CC-PMSM-v0 (fp32: 11 words = 44 B per env), bytes moved and the fraction of the H100 SXM data-sheet
@@ -14,6 +14,11 @@ the same future reference) packs the identities with the rows and adopts them wi
 that the candidates of every plant record identical reference trajectories until they terminate.  It then prints a fourth line:
   4. microseconds per env step of a fused rollout of --envs envs recording every step for 32 steps, auto-reset on, in three arms taking
      turns: shared coefficients, per-env parameter blocks that hold the shared parameters, and the same blocks with adopted identities.
+--params measures snapshots that carry the physical parameters (gemb200_pack_envs_params / gemb200_unpack_envs_params) instead, each
+line with a state-only arm (no parameter draws, gemb200_pack_envs / _unpack_envs) and a params arm (r_s, l_d, l_q, psi_p and j_rotor drawn
++-20 % at every reset; 192 B parameter row per env): 1. pack and 2. unpack of all envs, 3. fan-out of 1024 rows into all envs, and
+4. the MPC control step with rng="source" (identity only, shared plants) against rng="source", params="source" on randomised plants (the
+model handle draws from the same distribution).
 Run from the repository root after the build; writes nothing.
 """
 import argparse
@@ -63,6 +68,91 @@ def sim_of(n, seed=0):
     return VectorSim(cfg)
 
 
+DRAWN = ("r_s", "l_d", "l_q", "psi_p", "j_rotor")
+
+
+def randomised(sim):
+    """draw DRAWN +-20 % around the configuration's values at every reset of `sim`"""
+    from gym_electric_motor_b200 import _cabi as K
+
+    slots = [dict(r_s=K.MP_R_S, l_d=K.MP_L_D, l_q=K.MP_L_Q, psi_p=K.MP_PSI_P, j_rotor=K.MP_J_ROTOR)[x] for x in DRAWN]
+    v = [sim.cfg.motor_param[s] for s in slots]
+    sim.set_param_randomization(slots, [K.DIST_UNIFORM] * len(slots), [0.8 * x for x in v], [1.2 * x for x in v])
+    return sim
+
+
+def line(**kw):
+    for arm in ("state", "params"):
+        if f"bytes_{arm}" in kw and f"ms_{arm}" in kw:
+            kw[f"tb_s_{arm}"] = round(kw[f"bytes_{arm}"] / kw[f"ms_{arm}"] / 1e9, 3)
+            kw[f"frac_datasheet_{arm}"] = round(kw[f"bytes_{arm}"] / kw[f"ms_{arm}"] / 1e-3 / PEAK, 3)
+    print(json.dumps(kw))
+
+
+def params_main(args):
+    """--params: snapshots with physical parameters against state-only snapshots, and the MPC step on randomised plants"""
+    mode = args.rng
+    ids = mode == "source"
+    n, m = args.envs, 1024
+    state, drawn = sim_of(n, seed=0), randomised(sim_of(n, seed=0))
+    for s in (state, drawn):
+        s.reset()
+    words, _ = state.record_layout()
+    rec, idb, prb = 4 * words, (4 * 8 if ids else 0), 8 * 24  # state row, identity row, parameter row (bytes per env)
+    envp_b = 30 * 4  # fp32 envp column
+    snap_s, snap_p = state.snapshot(rng=ids), drawn.snapshot(rng=ids, params=True)
+    torch.cuda.synchronize()
+    ms_s = timed(lambda: state.snapshot(rng=ids), args.reps)
+    ms_p = timed(lambda: drawn.snapshot(rng=ids, params=True), args.reps)
+    line(what="pack", rng=mode, envs=n, ms_state=round(ms_s, 4), ms_params=round(ms_p, 4), bytes_state=2 * (rec + idb) * n,
+         bytes_params=2 * (rec + idb + prb) * n)
+    ms_s = timed(lambda: state.restore(snap_s, rng=mode), args.reps)
+    ms_p = timed(lambda: drawn.restore(snap_p, rng=mode, params="source"), args.reps)
+    # params: the rows read, 23 praw slots written, the pole-pair slot read, the envp column written
+    line(what="unpack", rng=mode, envs=n, ms_state=round(ms_s, 4), ms_params=round(ms_p, 4), bytes_state=2 * (rec + idb) * n,
+         bytes_params=2 * (rec + idb) * n + (prb + prb + envp_b) * n)
+    few_s, few_p = snap_s[:m], snap_p[:m]
+    ridx = torch.arange(m, device=state.device, dtype=torch.int32).repeat_interleave(n // m)
+    ms_s = timed(lambda: state.restore(few_s, rows=ridx, rng=mode), args.reps)
+    ms_p = timed(lambda: drawn.restore(few_p, rows=ridx, rng=mode, params="source"), args.reps)
+    b_s = (rec + 4) * n + rec * m + ((2 * idb + 4) * n + idb * m if ids else 0)
+    b_p = b_s + (prb + envp_b + 4) * n + prb * m  # 23 praw slots written + the pole-pair slot read, envp written, the row index again
+    line(what="fan_out_unpack", rng=mode, rows=m, envs=n, ms_state=round(ms_s, 4), ms_params=round(ms_p, 4), bytes_state=b_s, bytes_params=b_p)
+    del state, drawn, snap_s, snap_p, few_s, few_p
+    torch.cuda.empty_cache()
+
+    p_n, h = args.plants, args.horizon
+    c = n // p_n
+    out = dict(what="mpc_control_step_params", plants=p_n, candidates=c, horizon=h)
+    for arm in ("identity_only", "params_randomised"):
+        plant, model = sim_of(p_n, seed=1), sim_of(p_n * c, seed=2)
+        if arm == "params_randomised":
+            randomised(plant)
+            randomised(model)
+        plant.reset()
+        model.reset()
+        gen = torch.Generator(device=plant.device).manual_seed(0)
+        cand = (torch.rand((h, p_n * c, model.n_act), device=plant.device, generator=gen) * 2 - 1).contiguous()
+        rew = torch.empty((h, p_n * c), dtype=model.dtype, device=plant.device)
+        ridx = torch.arange(p_n, device=plant.device, dtype=torch.int32).repeat_interleave(c)
+        base = torch.arange(p_n, device=plant.device) * c
+        kw = dict(params=True) if arm == "params_randomised" else {}
+        kr = dict(params="source") if arm == "params_randomised" else {}
+
+        def control_step():
+            model.restore(plant.snapshot(rng=True, **kw), rows=ridx, rng="source", **kr)
+            model.rollout_into(cand, h, 1, None, None, rew, None)
+            plant.step(cand[0].index_select(0, rew.sum(0).view(p_n, c).argmax(1) + base))
+
+        ms = timed(control_step, args.reps)
+        out[f"ms_{arm}"] = round(ms, 4)
+        out[f"env_steps_per_s_{arm}"] = round(p_n * c * h / ms * 1e3, 1)
+        del plant, model, cand, rew
+        torch.cuda.empty_cache()
+    out["params_over_identity_only"] = round(out["ms_params_randomised"] / out["ms_identity_only"], 3)
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--envs", type=int, default=1 << 20)
@@ -70,9 +160,15 @@ def main():
     ap.add_argument("--plants", type=int, default=1024)
     ap.add_argument("--horizon", type=int, default=8)
     ap.add_argument("--rng", choices=("own", "source"), default="own")
+    ap.add_argument("--params", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: this benchmark measures the GPU and has no CPU fallback")
+    if args.params:
+        name, plimit = gpu_info()
+        print(f"GPU: {name}, power limit {plimit}")
+        params_main(args)
+        return
     ids = args.rng == "source"
     name, plimit = gpu_info()
     print(f"GPU: {name}, power limit {plimit}")
