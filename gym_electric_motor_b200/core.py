@@ -316,7 +316,9 @@ class ElectricMotorEnvironment(_EnvBase):
         reference envs with N `motor_parameter` / `load_parameter` dicts (electric_motor.py:118-131, polynomial_static_load.py:46-64).
         Both arguments are dicts  name -> array of N values  with the reference's parameter names (`r_s`, `l_d`, `psi_p`, `j_rotor`, ...;
         `a`, `b`, `c`, `j_load`); parameters that are not named keep the value the env was made with.  Limits, nominal values and the
-        normalisation stay those of the env.  `set_env_parameters()` without arguments returns to the shared parameters."""
+        normalisation stay those of the env.  `set_env_parameters()` without arguments returns to the shared parameters.  Pole pairs `p` may
+        be named only with the env's own value (ValueError otherwise: the angle increments are prepared per handle); the flux limits of an
+        induction motor's random initial states and the FluxObserver's constants stay those of the env's nominal motor (DESIGN.md §7)."""
         if self._scalar:
             raise TypeError("set_env_parameters() needs a batched environment (num_envs=...)")
         sim = self._ensure_sim()
@@ -334,6 +336,9 @@ class ElectricMotorEnvironment(_EnvBase):
             if name not in self._LP_SLOT:
                 raise KeyError(f"unknown load parameter {name!r}")
             lp[:, self._LP_SLOT[name]] = np.broadcast_to(np.asarray(vals, dtype=np.float64), (sim.n,))
+        from .randomization import check_pole_pairs
+
+        check_pole_pairs(mp[:, K.MP_P], cfg.motor_param[K.MP_P])
         sim.set_env_params(mp, lp)
 
     def randomize_env_parameters(self, motor_parameter=None, load_parameter=None):

@@ -972,6 +972,8 @@ int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const d
   for (size_t i = 0; i < n; ++i) {
     if (motor_param) std::memcpy(c.motor_param, motor_param + i * GEMB200_MAX_MOTOR_PARAM, sizeof(c.motor_param));
     if (load_param) std::memcpy(c.load_param, load_param + i * 8, sizeof(c.load_param));
+    if (c.motor_param[GEMB200_MP_P] != h->cfg.motor_param[GEMB200_MP_P])
+      return fail(GEMB200_E_INVALID, "pole pairs cannot differ per env: the angle increments are prepared on the host per handle");
     for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw[(size_t)s * n + i] = c.motor_param[s];
     for (int s = 0; s < 8; ++s) raw[(size_t)(GEMB200_MAX_MOTOR_PARAM + s) * n + i] = c.load_param[s];
     if (c.load_kind == GEMB200_LOAD_POLY_STATIC && !(c.load_param[GEMB200_LP_J_LOAD] + c.motor_param[GEMB200_MP_J_ROTOR] > 0))

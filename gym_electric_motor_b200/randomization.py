@@ -6,6 +6,8 @@ before any device call.
 """
 import math
 
+import numpy as np
+
 from . import _cabi as K
 
 DIST_KINDS = {"uniform": K.DIST_UNIFORM, "log_uniform": K.DIST_LOG_UNIFORM}
@@ -34,6 +36,15 @@ def parse_distribution(name, spec):
     if kind == "log_uniform" and lo <= 0:
         raise ValueError(f"{name}: log_uniform needs lo > 0")
     return DIST_KINDS[kind], lo, hi
+
+
+def check_pole_pairs(rows_p, pole_pairs):
+    """per-env rows (`set_env_parameters`, `VectorSim.set_env_params`) keep the handle's pole pairs: ValueError otherwise"""
+    rows_p = np.asarray(rows_p, dtype=np.float64)
+    bad = np.flatnonzero(rows_p != float(pole_pairs))
+    if bad.size:
+        raise ValueError(f"pole pairs 'p' cannot differ per env (env {int(bad[0])}: {rows_p[bad[0]]:g}, this env kind: {float(pole_pairs):g}): "
+                         "the angle increments are prepared per handle on the host")
 
 
 def encode_distributions(motor_parameter, load_parameter, mp_slot, lp_slot, flux_limits=False):

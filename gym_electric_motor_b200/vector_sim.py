@@ -125,9 +125,14 @@ class VectorSim:
 
     def set_env_params(self, motor_param=None, load_param=None):
         """Per-env parameter blocks (gemb200_set_env_params): motor_param [N, 16] / load_param [N, 8] float64 host arrays in the slot order of
-        `_cabi.MP_*` / `_cabi.LP_*`; None keeps the configuration's values; both None: back to the shared coefficients."""
+        `_cabi.MP_*` / `_cabi.LP_*`; None keeps the configuration's values; both None: back to the shared coefficients.  Every motor row must
+        keep the configuration's pole pairs (ValueError): the angle increments are prepared per handle."""
         mp = None if motor_param is None else np.ascontiguousarray(motor_param, dtype=np.float64).reshape(self.n, K.MAX_MOTOR_PARAM)
         lp = None if load_param is None else np.ascontiguousarray(load_param, dtype=np.float64).reshape(self.n, 8)
+        if mp is not None:
+            from .randomization import check_pole_pairs
+
+            check_pole_pairs(mp[:, K.MP_P], self.cfg.motor_param[K.MP_P])
         vp = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)  # noqa: E731
         K.check(self._lib.gemb200_set_env_params(self._h, vp(mp), vp(lp)), "gemb200_set_env_params")
         if mp is None and lp is None:

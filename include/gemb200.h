@@ -354,6 +354,9 @@ int gemb200_get_clock(gemb200_handle* h, uint64_t* call_id, uint64_t* n_steps, v
  * values).  The model coefficients are derived per env on the host exactly like the shared ones and live in a [30][N] device table that
  * every thread reads instead of the constant bank (36 B per PMSM env and launch; a fused rollout reads them once per K steps).  Limits,
  * nominal values, reward, constraints and references stay those of the configuration.  Both NULL: back to shared coefficients.
+ * Every motor row must keep the configuration's pole pairs (GEMB200_MP_P), else GEMB200_E_INVALID: the angle increments and the dq advance
+ * are prepared on the host per handle.  The flux limits of an induction motor with random initial states (init_im) and the FluxObserver
+ * constants (sop_param) stay the handle's as well.
  * Takes effect from the next reset / step; synchronises the device. */
 int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const double* load_param);
 
