@@ -298,6 +298,26 @@ class ElectricMotorEnvironment(_EnvBase):
             obs = obs.index_select(dim, self._filter_index)
         return (obs, ref), reward, terminated.view(torch.bool)
 
+    def rollout_returns(self, actions, discount=1.0, references=None):
+        """Score an action sequence: K steps with pre-computed actions [K, N, n_act] (SoA: [K, n_act, N]) in ONE kernel launch that hands
+        back each env's discounted return instead of its per-step rewards.  Returns (returns, end_step, (state, reference)):
+        end_step: int32 [N], the index of each env's first terminated step, K if it does not terminate within the launch;
+        returns: [N] in the env's dtype, sum of discount^k * reward_k over the steps up to and including that first termination (the
+        violation reward counts, nothing after it does, whatever the autoreset mode makes of the env afterwards);
+        (state, reference): the last step's outputs as `rollout(actions, record_every=0)` returns them, to bootstrap the envs with
+        end_step == K.  The env ends in exactly the state of `rollout(actions, references=references)`.  discount: finite, in [0, 1].
+        references: the reference feed of `rollout`.  Batched mode only; bad actions, discount or feed: ValueError before any launch."""
+        if self._scalar:
+            raise TypeError("rollout_returns() needs a batched environment (num_envs=...)")
+        sim = self._ensure_sim()
+        ret, end, (obs, ref) = sim.rollout_returns(actions, discount, references)
+        self._physical_system._k += int(actions.shape[0])
+        if not self._filter_identity:
+            if self._filter_index is None:
+                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
+            obs = obs.index_select(0 if sim.soa else 1, self._filter_index)
+        return ret, end, (obs, ref)
+
     def capture_steps(self, policy, n_steps, record=False, warmup=1, references=None):
         """`n_steps` closed-loop steps — action = policy(state, reference); env.step(action) — captured ONCE in a CUDA graph (graph.py);
         `.replay()` of the returned object runs them with a single call.  Batched mode only.  references: a static reference feed

@@ -701,9 +701,11 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
 // One launch over envs [begin, end) (end < 0: all).  new_call: this launch starts a new API call (fresh RNG call ids);
 // the chunks of one pipelined host step share them.  roll > 0: `roll` fused steps (rollout_kernel) whose call ids, step clock and
 // dead-time ring positions are exactly those of `roll` consecutive single-step calls; outputs every `every` steps (0: last only).
-// feed: the reference values of every step (StepParams::ref_feed), or NULL.
+// feed: the reference values of every step (StepParams::ref_feed), or NULL.  ret / ret_end / discount: the discounted returns of a
+// rollout (StepParams::ret_out), or NULL.
 static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, void* rew, uint8_t* term, cudaStream_t st,
-                   int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr) {
+                   int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr,
+                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
@@ -720,6 +722,7 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     p.roll_steps = roll; p.record_every = every;
     p.action = action; p.obs = (real*)obs; p.ref_out = (real*)ref; p.reward = (real*)rew; p.term = term;
     p.ref_feed = static_cast<const real*>(feed);
+    p.ret_out = static_cast<real*>(ret); p.ret_end = ret_end; p.discount = (real)discount;
     set_roll_strides(h, p);
     return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
   });
@@ -933,6 +936,18 @@ int gemb200_rollout_record_ref(gemb200_handle* h, const void* actions, const voi
   if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, record_every, references);
+}
+
+int gemb200_rollout_returns(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, double discount,
+                            void* return_out, int32_t* end_step_out, void* obs_out, void* ref_out, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (!return_out) return fail(GEMB200_E_INVALID, "return_out is NULL");
+  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
+  if (!(discount >= 0.0 && discount <= 1.0)) return fail(GEMB200_E_INVALID, "discount must be finite and in [0, 1]");
+  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  DeviceGuard guard(h->cfg.device);
+  return do_step(h, actions, obs_out, ref_out, nullptr, nullptr, (cudaStream_t)stream, 0, -1, true, n_steps, 0, references, return_out,
+                 end_step_out, discount);
 }
 
 int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, void* obs_out, void* ref_out, void* reward_out,

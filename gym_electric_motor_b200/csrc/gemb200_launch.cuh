@@ -11,7 +11,7 @@
 namespace gemb200 {
 
 // p.roll_steps == 0: one step (step_kernel); >= 1: that many fused steps (rollout_kernel).  A launch with a reference feed (p.ref_feed)
-// takes the general or ENVP instantiation: the PLAIN kernels have no feed.
+// or with discounted returns (p.ret_out) takes the general or ENVP instantiation: the PLAIN kernels have neither.
 template <int FAM, typename real> cudaError_t launch_step_f(bool finite, int nref, const StepParams<real>& p, cudaStream_t st);
 template <int FAM, typename real> cudaError_t launch_reset_f(int nref, const StepParams<real>& p, cudaStream_t st);
 
@@ -80,7 +80,7 @@ cudaError_t launch_step_f(bool finite, int nref, const StepParams<real>& p, cuda
 #define GEMB200_NREF(R)                                                                         \
   case R:                                                                                       \
     if constexpr (std::is_same<real, float>::value) {                                           \
-      if (p.plain && !p.ref_feed) return launch_plain_t<FAM, real, R>(finite, p, st);          \
+      if (p.plain && !p.ref_feed && !p.ret_out) return launch_plain_t<FAM, real, R>(finite, p, st); \
     }                                                                                           \
     if (p.layout == GEMB200_LAYOUT_SOA) return finite ? launch_step_t<FAM, true, real, R, true>(p, st) : launch_step_t<FAM, false, real, R, true>(p, st); \
     return finite ? launch_step_t<FAM, true, real, R, false>(p, st) : launch_step_t<FAM, false, real, R, false>(p, st);

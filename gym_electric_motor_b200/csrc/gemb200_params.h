@@ -265,6 +265,12 @@ struct StepParams {
   //      values of every step of this launch, [K][N][n_ref] (row-per-env) or [K][n_ref][N] (field-major).  Step k first overwrites the
   //      stored value of EVERY slot with row k, as gemb200_set_reference would.  nullptr: no feed ----
   const real* ref_feed;
+  // ---- discounted returns (gemb200_rollout_returns; rollout kernel, general and ENVP instantiations only, never PLAIN): per env
+  //      ret_out[i] = sum of discount^k * reward_k over the steps up to and including its first terminated one, ret_end[i] = the index
+  //      of that step (roll_steps if none; ret_end may be nullptr).  ret_out == nullptr: no returns ----
+  real* ret_out;
+  int32_t* ret_end;
+  real discount;
 };
 constexpr int kRngIdWords = 8;
 

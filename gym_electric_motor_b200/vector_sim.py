@@ -262,6 +262,54 @@ class VectorSim:
         K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(actions), _ptr(r), int(n_steps), int(record_every), _ptr(obs), _ptr(ref),
                                                      _ptr(rew), _ptr(term), self._stream()), "gemb200_rollout_record_ref")
 
+    def _as_actions(self, actions):
+        """check the actions of a fused launch: a contiguous device tensor of the action dtype, shaped [K, N, n_act] (SoA: [K, n_act, N])
+        with K >= 1.  Nothing is converted."""
+        if not isinstance(actions, torch.Tensor) or actions.dim() != 3:
+            raise ValueError(f"actions must be a [K, {', '.join(map(str, self._shape(self.n_act)))}] {self.act_dtype} tensor on {self.device}")
+        shape = (int(actions.shape[0]),) + self._shape(self.n_act)
+        if actions.dtype != self.act_dtype or actions.device != self.device or tuple(actions.shape) != shape:
+            raise ValueError(f"actions must be [K, {', '.join(map(str, shape[1:]))}] {self.act_dtype} on {self.device}, got "
+                             f"{tuple(actions.shape)} {actions.dtype} on {actions.device}")
+        if shape[0] < 1:
+            raise ValueError("a rollout needs K >= 1 steps")
+        if not actions.is_contiguous():
+            raise ValueError("actions must be contiguous")
+        return actions
+
+    @staticmethod
+    def _as_discount(discount):
+        g = float(discount)
+        if not (0.0 <= g <= 1.0):  # NaN fails both comparisons
+            raise ValueError(f"discount must be a finite number in [0, 1], got {discount!r}")
+        return g
+
+    def rollout_returns(self, actions, discount=1.0, references=None):
+        """K open-loop steps fused into ONE launch that hands back each env's discounted return instead of per-step outputs
+        (gemb200_rollout_returns).  Returns (returns [N] in the handle's dtype, end_step [N] int32, (obs, ref) of the last step):
+        end_step[i] = index of env i's first terminated step (K: none); returns[i] = sum of gamma^k * reward_k over k <= min(end_step, K - 1),
+        gamma = discount rounded to the handle's dtype.  The final state, clock and RNG position are those of
+        `rollout(actions, 1, references)`, bit for bit.  actions: [K, N, n_act] (SoA: [K, n_act, N]) in the action dtype on the device;
+        references: the reference feed of `rollout`.  Bad actions, discount or feed: ValueError before any launch."""
+        a = self._as_actions(actions)
+        k = int(a.shape[0])
+        g = self._as_discount(discount)
+        r = None if references is None else self._as_feed(references, k)
+        obs, ref, _, _ = self._alloc_outputs()
+        ret = torch.empty(self.n, dtype=self.dtype, device=self.device)
+        end = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        K.check(self._lib.gemb200_rollout_returns(self._h, _ptr(a), _ptr(r), k, g, _ptr(ret), _ptr(end), _ptr(obs), _ptr(ref) if self.n_ref else None,
+                                                  self._stream()), "gemb200_rollout_returns")
+        return ret, end, (obs, ref)
+
+    def rollout_returns_into(self, actions, n_steps, discount, ret, end=None, obs=None, ref=None, references=None):
+        """Raw variant of `rollout_returns` for benchmarking: caller-owned outputs (all but `ret` may be None), no allocation, no
+        conversion.  The discount and the reference feed are checked like there."""
+        g = self._as_discount(discount)
+        r = None if references is None else self._as_feed(references, n_steps)
+        K.check(self._lib.gemb200_rollout_returns(self._h, _ptr(actions), _ptr(r), int(n_steps), g, _ptr(ret), _ptr(end), _ptr(obs),
+                                                  _ptr(ref) if self.n_ref else None, self._stream()), "gemb200_rollout_returns")
+
     # ------------------------------------------------------------------ host-buffer API (numpy)
     def step_host(self, action, out=None):
         """Same step through HOST buffers (the C-ABI does H2D, launch, D2H, sync).  `out` = tuple of numpy arrays to

@@ -320,6 +320,21 @@ int gemb200_rollout_record(gemb200_handle* h, const void* actions, int32_t n_ste
 int gemb200_rollout_record_ref(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t record_every,
                                void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream);
 
+/* Discounted returns of a fused rollout: n_steps >= 1 steps in ONE launch, scored in registers.  Per env i, with gamma = discount rounded
+ * to the handle's dtype:
+ *   end_step_out[i] (int32, [N]) = the 0-based index of the env's first step with terminated = 1, or n_steps if there is none;
+ *   return_out[i] ([N], the handle's dtype) = sum of gamma^k * reward_k over k = 0 .. min(end_step, n_steps - 1): the terminating step's
+ *   reward counts, nothing after it does, whatever the auto-reset mode does to the env afterwards.  Computed as w = 1, G = 0; per step
+ *   G = G + (w * r_k) while not yet terminated, then w = w * gamma; two roundings per update, no FMA.
+ * obs_out / ref_out take the LAST step's outputs as gemb200_rollout_record(record_every = 0) writes them.  The final state, clock and
+ * RNG position are exactly those of gemb200_rollout_record_ref with the same arguments.  references: the reference feed of
+ * gemb200_rollout_record_ref, or NULL.  end_step_out, obs_out, ref_out may be NULL; return_out may not.  The returns and end steps go to the
+ * caller's buffers only: bound peers (gemb200_bind_peers) do not gather them.  Stream-ordered, capturable in a
+ * CUDA graph under the device clock.  GEMB200_E_INVALID: NULL handle or return_out, n_steps out of [1, 2^24], a discount that is not a
+ * finite number in [0, 1], a feed into a configuration with n_ref == 0. */
+int gemb200_rollout_returns(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, double discount,
+                            void* return_out, int32_t* end_step_out, void* obs_out, void* ref_out, void* stream);
+
 /* OdeSolver.y / set_initial_value (physical_systems/solvers.py:4-76): ODE state as double [N][n_ode]
  * (AoS, device), angle unwrapped to (-pi, pi].  Used for checkpointing and oracle injection. */
 int gemb200_get_ode_state(gemb200_handle* h, double* ode_out, void* stream);
