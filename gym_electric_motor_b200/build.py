@@ -3,7 +3,8 @@
     python -m gym_electric_motor_b200.build [--force] [--verbose]
 
 The step kernel's 200 instantiations are spread over twelve translation units (motor family x real, csrc/gemb200_step_tu.cu)
-that compile in parallel; objects go to build/ (git-ignored), only the linked .so stays in the package.
+that compile in parallel, and the rollout-Jacobian kernels over twelve more (csrc/gemb200_jac_tu.cu); objects go to build/ (git-ignored),
+only the linked .so stays in the package.
 """
 import hashlib
 import os
@@ -14,8 +15,9 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 HEADERS = [os.path.join(CSRC, "gemb200_kernels.cuh"), os.path.join(CSRC, "gemb200_params.h"), os.path.join(CSRC, "gemb200_launch.cuh"),
-           os.path.join(CSRC, "gemb200_model.h"), os.path.join(HERE, "..", "include", "gemb200.h")]
-SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu")]
+           os.path.join(CSRC, "gemb200_model.h"), os.path.join(CSRC, "gemb200_jac.h"), os.path.join(CSRC, "gemb200_tangent.cuh"),
+           os.path.join(HERE, "..", "include", "gemb200.h")]
+SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu"), os.path.join(CSRC, "gemb200_jac_tu.cu")]
 OUT = os.path.join(HERE, "libgemb200.so")
 OBJ_DIR = os.path.join(HERE, "..", "build", "gemb200")
 # -fmad=false: no implicit contraction of a*b+c — every fused multiply-add of the kernels is written out (fm() in gemb200_kernels.cuh), so
@@ -50,6 +52,10 @@ def _units(only=None):
             if only and (fam, real) not in only:
                 continue
             units.append((f"step_f{fam}_{real}", SOURCES[1], [f"-DGEMB200_TU_FAM={fam}", f"-DGEMB200_TU_REAL={real}"] + (LINEINFO if real == "float" else [])))
+    if not only:  # the rollout-Jacobian kernels (gemb200_jac_tu.cu): one unit per family x real, like the step kernels
+        for fam in FAMILIES:
+            for real in REALS:
+                units.append((f"jac_f{fam}_{real}", SOURCES[2], [f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
     return units
 
 

@@ -318,6 +318,26 @@ class ElectricMotorEnvironment(_EnvBase):
             obs = obs.index_select(0 if sim.soa else 1, self._filter_index)
         return ret, end, (obs, ref)
 
+    def rollout_jacobians(self, actions, references=None):
+        """Linearise the plant along an action sequence: K steps with pre-computed actions [K, N, n_act] in ONE kernel launch that also
+        returns, per step k and env i, jac_x[k, i] = d x_{k+1} / d x_k ([n_x, n_x]) and jac_u[k, i] = d x_{k+1} / d a_k ([n_x, n_u]; None
+        for finite converters).  x is the ODE state of `get_ode_state` ([load states | motor states], the angle last, in radians), a the
+        action as passed to `step`.  Returns ((jac_x, jac_u), ((states, references), rewards, terminateds)), the second part exactly as
+        `rollout(actions, record_every=1, references=references)` returns it; the env ends in that call's state.  A terminating step reports
+        the Jacobian of the physical step it took.  `calc_jacobian` does not switch this on or off.  Refused configurations (dead time, RC
+        supply, dq actions on the observer angle, SoA): NotImplementedError (DESIGN.md §7).
+        Batched mode only; bad actions or feed: ValueError before any launch."""
+        if self._scalar:
+            raise TypeError("rollout_jacobians() needs a batched environment (num_envs=...)")
+        sim = self._ensure_sim()
+        (jx, ju), (obs, ref, reward, terminated) = sim.rollout_jacobians(actions, references)
+        self._physical_system._k += int(actions.shape[0])
+        if not self._filter_identity:
+            if self._filter_index is None:
+                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
+            obs = obs.index_select(2, self._filter_index)
+        return (jx, ju), ((obs, ref), reward, terminated.view(torch.bool))
+
     def capture_steps(self, policy, n_steps, record=False, warmup=1, references=None):
         """`n_steps` closed-loop steps — action = policy(state, reference); env.step(action) — captured ONCE in a CUDA graph (graph.py);
         `.replay()` of the returned object runs them with a single call.  Batched mode only.  references: a static reference feed

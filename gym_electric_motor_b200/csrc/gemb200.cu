@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 
+#include "gemb200_jac.h"
 #include "gemb200_launch.cuh"
 
 using namespace gemb200;
@@ -659,6 +660,23 @@ static cudaError_t launch_reset(int fam, int nref, const StepParams<real>& p, cu
 }
 
 template <typename real>
+static cudaError_t launch_jac(int fam, bool finite, int nref, const StepParams<real>& p, const JacOut& jo, cudaStream_t st) {
+#ifdef GEMB200_ONLY_FAM
+  return cudaErrorInvalidValue;
+#else
+  switch (fam) {
+    case kDC1: return launch_jac_f<kDC1, real>(finite, nref, p, jo, st);
+    case kDC2: return launch_jac_f<kDC2, real>(finite, nref, p, jo, st);
+    case kSYNC: return launch_jac_f<kSYNC, real>(finite, nref, p, jo, st);
+    case kEESM: return launch_jac_f<kEESM, real>(finite, nref, p, jo, st);
+    case kSCIM: return launch_jac_f<kSCIM, real>(finite, nref, p, jo, st);
+    case kDFIM: return launch_jac_f<kDFIM, real>(finite, nref, p, jo, st);
+  }
+  return cudaErrorInvalidValue;
+#endif
+}
+
+template <typename real>
 static void set_roll_strides(const gemb200_handle* h, StepParams<real>& p) {
   const int64_t n = h->cfg.n_envs;
   p.out_has = (p.obs ? 1 : 0) | ((p.ref_out && h->n_ref > 0) ? 2 : 0) | (p.reward ? 4 : 0) | (p.term ? 8 : 0);
@@ -702,10 +720,11 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
 // the chunks of one pipelined host step share them.  roll > 0: `roll` fused steps (rollout_kernel) whose call ids, step clock and
 // dead-time ring positions are exactly those of `roll` consecutive single-step calls; outputs every `every` steps (0: last only).
 // feed: the reference values of every step (StepParams::ref_feed), or NULL.  ret / ret_end / discount: the discounted returns of a
-// rollout (StepParams::ret_out), or NULL.
+// rollout (StepParams::ret_out), or NULL.  jac: the Jacobian outputs of gemb200_rollout_jacobians, or NULL; with them the launch takes the
+// rollout-Jacobian kernel (gemb200_tangent.cuh) instead of the step / rollout kernels.
 static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, void* rew, uint8_t* term, cudaStream_t st,
                    int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr,
-                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0) {
+                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const JacOut* jac = nullptr) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
@@ -724,6 +743,7 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     p.ref_feed = static_cast<const real*>(feed);
     p.ret_out = static_cast<real*>(ret); p.ret_end = ret_end; p.discount = (real)discount;
     set_roll_strides(h, p);
+    if (jac) return launch_jac<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, *jac, st);
     return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
   });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string(roll > 0 ? "rollout launch: " : "step launch: ") + cudaGetErrorString(e));
@@ -820,6 +840,27 @@ int gemb200_query_dims(const gemb200_config* cfg, int32_t* n_state, int32_t* n_o
   if (n_ode) *n_ode = d.n_ode;
   if (n_act) *n_act = d.n_act;
   if (n_ref) *n_ref = cfg->n_ref;
+  return GEMB200_OK;
+}
+
+// Configurations whose rollout Jacobians the library does not compute (DESIGN.md §7, "Rollout Jacobians"): the reason, or nullptr
+static const char* jacobian_refusal(const gemb200_config* c) {
+  if (c->dead_time_steps > 0) return "rollout Jacobians: a dead time is refused, the action enters through the queue, which is not part of the ODE state (DESIGN.md §7)";
+  if (c->supply_kind == GEMB200_SUPPLY_RC) return "rollout Jacobians: the RC supply is refused, its state couples through i_sup and is not part of the ODE state (DESIGN.md §7)";
+  if (c->action_dq == 2 || c->action_dq == 3)
+    return "rollout Jacobians: dq actions on the FluxObserver angle are refused, the control path reads an observer state that is not part of the ODE state (DESIGN.md §7)";
+  if (c->layout == GEMB200_LAYOUT_SOA) return "rollout Jacobians: the SoA layout is refused, the launch writes row-per-env outputs only (DESIGN.md §7)";
+  return nullptr;
+}
+
+int gemb200_query_jacobian_dims(const gemb200_config* cfg, int32_t* n_x, int32_t* n_u) {
+  if (!cfg) return fail(GEMB200_E_INVALID, "config is NULL");
+  Dims d;
+  int rc = derive_dims(cfg, &d);
+  if (rc) return rc;
+  if (const char* why = jacobian_refusal(cfg)) return fail(GEMB200_E_INVALID, why);
+  if (n_x) *n_x = d.n_ode;
+  if (n_u) *n_u = cfg->finite ? 0 : d.n_act;
   return GEMB200_OK;
 }
 
@@ -948,6 +989,19 @@ int gemb200_rollout_returns(gemb200_handle* h, const void* actions, const void* 
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, nullptr, nullptr, (cudaStream_t)stream, 0, -1, true, n_steps, 0, references, return_out,
                  end_step_out, discount);
+}
+
+int gemb200_rollout_jacobians(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, void* jac_x_out, void* jac_u_out,
+                              void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (const char* why = jacobian_refusal(&h->cfg)) return fail(GEMB200_E_INVALID, why);
+  if (!jac_x_out) return fail(GEMB200_E_INVALID, "jac_x_out is NULL");
+  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
+  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  const JacOut jo{jac_x_out, h->cfg.finite ? nullptr : jac_u_out, h->cfg.finite ? 0 : h->n_act};
+  DeviceGuard guard(h->cfg.device);
+  return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
+                 1.0, &jo);
 }
 
 int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, void* obs_out, void* ref_out, void* reward_out,

@@ -310,6 +310,42 @@ class VectorSim:
         K.check(self._lib.gemb200_rollout_returns(self._h, _ptr(actions), _ptr(r), int(n_steps), g, _ptr(ret), _ptr(end), _ptr(obs),
                                                   _ptr(ref) if self.n_ref else None, self._stream()), "gemb200_rollout_returns")
 
+    def jacobian_dims(self):
+        """(n_x, n_u) of `rollout_jacobians`: n_x = n_ode, n_u = n_act (0 for finite converters).  NotImplementedError for a configuration the
+        launch refuses (DESIGN.md §7)."""
+        lib = K.load_library()  # a configuration query: no handle, no launch
+        nx, nu = C.c_int32(), C.c_int32()
+        if lib.gemb200_query_jacobian_dims(C.byref(self.cfg), C.byref(nx), C.byref(nu)):
+            raise NotImplementedError(lib.gemb200_last_error().decode())
+        return nx.value, nu.value
+
+    def rollout_jacobians(self, actions, references=None):
+        """K open-loop steps in ONE launch that also linearise the plant (gemb200_rollout_jacobians).  Returns ((jac_x, jac_u), (obs, ref, rew,
+        term)): jac_x [K, N, n_x, n_x] = d x_{k+1} / d x_k, jac_u [K, N, n_x, n_u] = d x_{k+1} / d a_k (None when n_u == 0), both in the
+        handle's dtype, x = the ODE state of `get_ode_state` (the angle in radians), a = the caller's action; the outputs of every step exactly
+        as `rollout(actions, record_every=1, references=references)` returns them, and the same final state, clock and RNG position.
+        Refused configurations: NotImplementedError (DESIGN.md §7); bad actions or feed: ValueError before any launch."""
+        nx, nu = self.jacobian_dims()
+        a = self._as_actions(actions)
+        k = int(a.shape[0])
+        r = None if references is None else self._as_feed(references, k)
+        jx = torch.empty((k, self.n, nx, nx), dtype=self.dtype, device=self.device)
+        ju = torch.empty((k, self.n, nx, nu), dtype=self.dtype, device=self.device) if nu else None
+        obs = torch.empty((k,) + self._shape(self.n_state), dtype=self.dtype, device=self.device)
+        ref = torch.empty((k,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device)
+        rew = torch.empty((k, self.n), dtype=self.dtype, device=self.device)
+        term = torch.empty((k, self.n), dtype=torch.uint8, device=self.device)
+        self.rollout_jacobians_into(a, k, jx, ju, obs, ref, rew, term, r)
+        return (jx, ju), (obs, ref, rew, term)
+
+    def rollout_jacobians_into(self, actions, n_steps, jac_x, jac_u=None, obs=None, ref=None, rew=None, term=None, references=None):
+        """Raw variant of `rollout_jacobians` for benchmarking: caller-owned outputs (all but `jac_x` may be None), no allocation, no
+        conversion.  The reference feed is checked like there."""
+        r = None if references is None else self._as_feed(references, n_steps)
+        K.check(self._lib.gemb200_rollout_jacobians(self._h, _ptr(actions), _ptr(r), int(n_steps), _ptr(jac_x), _ptr(jac_u), _ptr(obs),
+                                                    _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term), self._stream()),
+                "gemb200_rollout_jacobians")
+
     # ------------------------------------------------------------------ host-buffer API (numpy)
     def step_host(self, action, out=None):
         """Same step through HOST buffers (the C-ABI does H2D, launch, D2H, sync).  `out` = tuple of numpy arrays to

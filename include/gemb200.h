@@ -335,6 +335,23 @@ int gemb200_rollout_record_ref(gemb200_handle* h, const void* actions, const voi
 int gemb200_rollout_returns(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, double discount,
                             void* return_out, int32_t* end_step_out, void* obs_out, void* ref_out, void* stream);
 
+/* The linearised plant along a fused rollout (SCMLSystem._system_jacobian, physical_systems.py:238, integrated over each step).
+ * gemb200_query_jacobian_dims: n_x = n_ode (the state of gemb200_get_ode_state: [load states | motor states], the angle last, in radians)
+ * and n_u = n_act (0 for finite converters: their actions are integers).  Needs no GPU.  GEMB200_E_INVALID for every configuration the
+ * launch refuses (DESIGN.md §7): a dead time, the RC supply, dq actions on the FluxObserver angle (action_dq = 2, 3), the SoA layout.
+ * gemb200_rollout_jacobians: n_steps >= 1 open-loop steps in ONE launch.  Per step k and env i
+ *   jac_x_out[k][i] = d x_{k+1} / d x_k  ([n_x][n_x], row-major),   jac_u_out[k][i] = d x_{k+1} / d a_k  ([n_x][n_u]),
+ * a = the caller's action as passed to gemb200_step; both in the handle's dtype, [K][N][n_x][..].  At non-smooth points the derivative is
+ * the one-sided one of the branch the step took (clipped duty cycle: 0; interlocking and current-sign voltages: 0; angle wrap: 1).  A
+ * terminating step reports the Jacobian of the physical step it took; terminated_out tells which rows precede an auto-reset.
+ * obs_out / ref_out / reward_out / terminated_out receive exactly what gemb200_rollout_record_ref(record_every = 1) writes, and the final
+ * state, clock and RNG position are those of that call.  references: its reference feed, or NULL.  Any output may be NULL except
+ * jac_x_out; jac_u_out is ignored when n_u == 0.  The Jacobians go to the caller's buffers only: bound peers do not gather them.
+ * Stream-ordered, capturable in a CUDA graph under the device clock. */
+int gemb200_query_jacobian_dims(const gemb200_config* cfg, int32_t* n_x, int32_t* n_u);
+int gemb200_rollout_jacobians(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, void* jac_x_out, void* jac_u_out,
+                              void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream);
+
 /* OdeSolver.y / set_initial_value (physical_systems/solvers.py:4-76): ODE state as double [N][n_ode]
  * (AoS, device), angle unwrapped to (-pi, pi].  Used for checkpointing and oracle injection. */
 int gemb200_get_ode_state(gemb200_handle* h, double* ode_out, void* stream);
