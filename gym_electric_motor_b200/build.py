@@ -3,7 +3,8 @@
     python -m gym_electric_motor_b200.build [--force] [--verbose]
 
 The step kernel's 200 instantiations are spread over twelve translation units (motor family x real, csrc/gemb200_step_tu.cu)
-that compile in parallel, and the rollout-Jacobian kernels over twelve more (csrc/gemb200_jac_tu.cu); objects go to build/ (git-ignored),
+that compile in parallel, the rollout-Jacobian kernels over twelve more (csrc/gemb200_jac_tu.cu) and the return-gradient kernels over another twelve
+(csrc/gemb200_grad_tu.cu); objects go to build/ (git-ignored),
 only the linked .so stays in the package.
 """
 import hashlib
@@ -17,7 +18,8 @@ CSRC = os.path.join(HERE, "csrc")
 HEADERS = [os.path.join(CSRC, "gemb200_kernels.cuh"), os.path.join(CSRC, "gemb200_params.h"), os.path.join(CSRC, "gemb200_launch.cuh"),
            os.path.join(CSRC, "gemb200_model.h"), os.path.join(CSRC, "gemb200_jac.h"), os.path.join(CSRC, "gemb200_tangent.cuh"),
            os.path.join(HERE, "..", "include", "gemb200.h")]
-SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu"), os.path.join(CSRC, "gemb200_jac_tu.cu")]
+SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu"), os.path.join(CSRC, "gemb200_jac_tu.cu"),
+           os.path.join(CSRC, "gemb200_grad_tu.cu")]
 OUT = os.path.join(HERE, "libgemb200.so")
 OBJ_DIR = os.path.join(HERE, "..", "build", "gemb200")
 # -fmad=false: no implicit contraction of a*b+c — every fused multiply-add of the kernels is written out (fm() in gemb200_kernels.cuh), so
@@ -56,6 +58,9 @@ def _units(only=None):
         for fam in FAMILIES:
             for real in REALS:
                 units.append((f"jac_f{fam}_{real}", SOURCES[2], [f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
+        for fam in FAMILIES:  # the return-gradient kernels (gemb200_grad_tu.cu), likewise
+            for real in REALS:
+                units.append((f"grad_f{fam}_{real}", SOURCES[3], [f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
     return units
 
 

@@ -338,6 +338,40 @@ class ElectricMotorEnvironment(_EnvBase):
             obs = obs.index_select(2, self._filter_index)
         return (jx, ju), ((obs, ref), reward, terminated.view(torch.bool))
 
+    def rollout_return_grads(self, actions, discount=1.0, references=None, value_grad=None):
+        """Score an action sequence and differentiate the score: `rollout_returns` plus, from the same launch, grad_a [K, N, n_u] =
+        d returns[i] / d a_k[i] (a = the action as passed to `step`, dq actions included; exactly 0 for k >= end_step[i]) and grad_x0 [N, n_x]
+        = d returns[i] / d x_0[i] (x = the ODE state of `get_ode_state`, the angle last, in radians).  Returns (returns, end_step,
+        (state, reference), grad_a, grad_x0), the first three as `rollout_returns(actions, discount, references)` returns them; the env
+        ends in that call's state.  value_grad [N, n_x] (env dtype): the gradient of a bootstrap value V(x_K), added as discount^K *
+        value_grad[i] to the adjoint of the envs with end_step == K (returns itself does not include V).  Non-smooth points take the
+        one-sided derivative of the branch the step took, and termination has derivative 0: the gradient does not see a constraint a
+        perturbed sequence would hit (DESIGN.md §7).  Refused configurations (those of `rollout_jacobians`, finite converters, a reward on
+        an entry a state wrapper appends): NotImplementedError.  Batched mode only; bad actions, discount, feed or value_grad: ValueError
+        before any launch."""
+        if self._scalar:
+            raise TypeError("rollout_return_grads() needs a batched environment (num_envs=...)")
+        sim = self._ensure_sim()
+        ret, end, (obs, ref), ga, gx = sim.rollout_return_grads(actions, discount, references, value_grad)
+        self._physical_system._k += int(actions.shape[0])
+        if not self._filter_identity:
+            if self._filter_index is None:
+                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
+            obs = obs.index_select(1, self._filter_index)
+        return ret, end, (obs, ref), ga, gx
+
+    def differentiable_returns(self, actions, discount=1.0, references=None):
+        """`rollout_returns(actions, discount, references)[0]` as a torch autograd function of `actions`: the forward pass runs ONE
+        `rollout_return_grads` launch and ADVANCES the env by K steps like `rollout_returns`; the backward pass returns
+        grad_output[None, :, None] * grad_a.  So an action sequence that is an `nn.Parameter`, or the output of a policy, can be optimised
+        with a torch optimiser.  Every call starts from the env's current state: to evaluate the same start again, branch the envs first
+        (`snapshot_envs`) and put them back with `restore_envs(..., rng="source")` before the next call."""
+        if self._scalar:
+            raise TypeError("differentiable_returns() needs a batched environment (num_envs=...)")
+        if not isinstance(actions, torch.Tensor):
+            raise ValueError(f"actions must be a torch tensor, got {type(actions).__name__}")
+        return _DifferentiableReturns.apply(actions, self, discount, references)
+
     def capture_steps(self, policy, n_steps, record=False, warmup=1, references=None):
         """`n_steps` closed-loop steps — action = policy(state, reference); env.step(action) — captured ONCE in a CUDA graph (graph.py);
         `.replay()` of the returned object runs them with a single call.  Batched mode only.  references: a static reference feed
@@ -497,3 +531,18 @@ class ElectricMotorEnvironment(_EnvBase):
             self._sim.close()
             self._sim = None
         self._physical_system.attach(None)
+
+
+class _DifferentiableReturns(torch.autograd.Function):
+    """returns = env.rollout_return_grads(actions, ...)[0]; d returns / d actions from the same launch"""
+
+    @staticmethod
+    def forward(ctx, actions, env, discount, references):
+        ret, _, _, ga, _ = env.rollout_return_grads(actions.detach(), discount, references)
+        ctx.save_for_backward(ga)
+        return ret
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        (ga,) = ctx.saved_tensors
+        return grad_output[None, :, None] * ga, None, None, None

@@ -677,6 +677,23 @@ static cudaError_t launch_jac(int fam, bool finite, int nref, const StepParams<r
 }
 
 template <typename real>
+static cudaError_t launch_grad(int fam, int nref, const StepParams<real>& p, const GradOut& go, cudaStream_t st) {
+#ifdef GEMB200_ONLY_FAM
+  return cudaErrorInvalidValue;
+#else
+  switch (fam) {
+    case kDC1: return launch_grad_f<kDC1, real>(nref, p, go, st);
+    case kDC2: return launch_grad_f<kDC2, real>(nref, p, go, st);
+    case kSYNC: return launch_grad_f<kSYNC, real>(nref, p, go, st);
+    case kEESM: return launch_grad_f<kEESM, real>(nref, p, go, st);
+    case kSCIM: return launch_grad_f<kSCIM, real>(nref, p, go, st);
+    case kDFIM: return launch_grad_f<kDFIM, real>(nref, p, go, st);
+  }
+  return cudaErrorInvalidValue;
+#endif
+}
+
+template <typename real>
 static void set_roll_strides(const gemb200_handle* h, StepParams<real>& p) {
   const int64_t n = h->cfg.n_envs;
   p.out_has = (p.obs ? 1 : 0) | ((p.ref_out && h->n_ref > 0) ? 2 : 0) | (p.reward ? 4 : 0) | (p.term ? 8 : 0);
@@ -721,10 +738,11 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
 // dead-time ring positions are exactly those of `roll` consecutive single-step calls; outputs every `every` steps (0: last only).
 // feed: the reference values of every step (StepParams::ref_feed), or NULL.  ret / ret_end / discount: the discounted returns of a
 // rollout (StepParams::ret_out), or NULL.  jac: the Jacobian outputs of gemb200_rollout_jacobians, or NULL; with them the launch takes the
-// rollout-Jacobian kernel (gemb200_tangent.cuh) instead of the step / rollout kernels.
+// rollout-Jacobian kernel (gemb200_tangent.cuh) instead of the step / rollout kernels.  grad: the outputs of gemb200_rollout_return_grads,
+// or NULL; with them the launch takes the return-gradient kernel (gemb200_tangent.cuh).
 static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, void* rew, uint8_t* term, cudaStream_t st,
                    int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr,
-                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const JacOut* jac = nullptr) {
+                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const JacOut* jac = nullptr, const GradOut* grad = nullptr) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
@@ -744,6 +762,7 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     p.ret_out = static_cast<real*>(ret); p.ret_end = ret_end; p.discount = (real)discount;
     set_roll_strides(h, p);
     if (jac) return launch_jac<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, *jac, st);
+    if (grad) return launch_grad<real>(h->fam, h->n_ref, p, *grad, st);
     return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
   });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string(roll > 0 ? "rollout launch: " : "step launch: ") + cudaGetErrorString(e));
@@ -861,6 +880,51 @@ int gemb200_query_jacobian_dims(const gemb200_config* cfg, int32_t* n_x, int32_t
   if (const char* why = jacobian_refusal(cfg)) return fail(GEMB200_E_INVALID, why);
   if (n_x) *n_x = d.n_ode;
   if (n_u) *n_u = cfg->finite ? 0 : d.n_act;
+  return GEMB200_OK;
+}
+
+// The entry of the family's state vector (before the wrappers) behind each entry of the observation row, or -1 for an entry a wrapper
+// appends (CosSin, FluxObserver, CurrentSum); returns the row width
+static int row_bases(const gemb200_config* c, int n_state, int8_t (&base)[GEMB200_MAX_STATE]) {
+  int w = n_state;
+  for (int j = 0; j < GEMB200_MAX_STATE; ++j) base[j] = j < n_state ? (int8_t)j : (int8_t)-1;
+  for (int k = 0; k < c->n_state_ops; ++k) {
+    switch (c->sop_kind[k]) {
+      case GEMB200_SOP_COS_SIN:
+        if (c->sop_idx[k][1]) { for (int j = c->sop_idx[k][0]; j < w - 1; ++j) base[j] = base[j + 1]; --w; }  // remove_angle
+        base[w] = base[w + 1] = -1;
+        w += 2;
+        break;
+      case GEMB200_SOP_FLUX_OBSERVER: base[w] = base[w + 1] = -1; w += 2; break;
+      case GEMB200_SOP_CURRENT_SUM: base[w] = -1; w += 1; break;
+      default: break;  // state noise: additive, the entry keeps its base
+    }
+  }
+  return w;
+}
+
+// Configurations whose return gradients the library does not compute (DESIGN.md §7, "Return gradients"): the reason, or nullptr.
+// Call after derive_dims succeeded.
+static const char* return_grad_refusal(const gemb200_config* c, const Dims& d) {
+  if (const char* why = jacobian_refusal(c)) return why;
+  if (c->finite) return "return gradients: finite converters are refused, their actions are integers without a derivative (DESIGN.md §7)";
+  int8_t base[GEMB200_MAX_STATE];
+  const int w = row_bases(c, d.n_state, base);
+  for (int j = 0; j < w; ++j)
+    if (c->reward_weight[j] != 0.0 && base[j] < 0)
+      return "return gradients: the reward weights an entry a state wrapper appends (CosSin, FluxObserver, CurrentSum), which is not a function of the ODE state in the tangent pass (DESIGN.md §7)";
+  return nullptr;
+}
+
+int gemb200_query_return_grad_dims(const gemb200_config* cfg, int32_t* n_x, int32_t* n_u, int32_t* ws_words) {
+  if (!cfg) return fail(GEMB200_E_INVALID, "config is NULL");
+  Dims d;
+  int rc = derive_dims(cfg, &d);
+  if (rc) return rc;
+  if (const char* why = return_grad_refusal(cfg, d)) return fail(GEMB200_E_INVALID, why);
+  if (n_x) *n_x = d.n_ode;
+  if (n_u) *n_u = d.n_act;
+  if (ws_words) *ws_words = d.n_ode * (d.n_ode + d.n_act) + d.n_ode + d.n_act;
   return GEMB200_OK;
 }
 
@@ -1002,6 +1066,42 @@ int gemb200_rollout_jacobians(gemb200_handle* h, const void* actions, const void
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
                  1.0, &jo);
+}
+
+int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, double discount, const void* value_grad,
+                                 void* workspace, uint64_t workspace_bytes, void* return_out, int32_t* end_step_out, void* grad_a_out, void* grad_x0_out,
+                                 void* obs_out, void* ref_out, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  Dims d;
+  derive_dims(&h->cfg, &d);
+  if (const char* why = return_grad_refusal(&h->cfg, d)) return fail(GEMB200_E_INVALID, why);
+  if (!return_out) return fail(GEMB200_E_INVALID, "return_out is NULL");
+  if (!grad_a_out) return fail(GEMB200_E_INVALID, "grad_a_out is NULL");
+  if (!grad_x0_out) return fail(GEMB200_E_INVALID, "grad_x0_out is NULL");
+  if (!workspace) return fail(GEMB200_E_INVALID, "workspace is NULL");
+  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
+  if (!(discount >= 0.0 && discount <= 1.0)) return fail(GEMB200_E_INVALID, "discount must be finite and in [0, 1]");
+  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  const uint64_t words = (uint64_t)(d.n_ode * (d.n_ode + d.n_act) + d.n_ode + d.n_act);
+  const uint64_t need = (uint64_t)n_steps * (uint64_t)h->cfg.n_envs * words * (uint64_t)h->rsz;
+  if (workspace_bytes < need) return fail(GEMB200_E_INVALID, "workspace too small: it needs n_steps * n_envs * ws_words * sizeof(real) bytes (gemb200_query_return_grad_dims)");
+  GradOut go{};
+  go.ws = workspace; go.grad_a = grad_a_out; go.grad_x0 = grad_x0_out; go.value_grad = value_grad; go.nu = h->n_act;
+  {  // the state-vector entry behind every reward term, in fill_params' order of the terms
+    int8_t base[GEMB200_MAX_STATE];
+    const int w = row_bases(&h->cfg, d.n_state, base);
+    int t = 0;
+    for (int j = 0; j < w; ++j) {
+      if (h->cfg.reward_weight[j] == 0.0) continue;
+      int slot = -1;
+      for (int r = 0; r < h->cfg.n_ref; ++r) if (h->cfg.ref_state[r] == j) slot = r;
+      if (slot >= 0) go.ref_base[slot] = base[j]; else go.rw_base[t++] = base[j];
+      go.wmask |= 1u << base[j];
+    }
+  }
+  DeviceGuard guard(h->cfg.device);
+  return do_step(h, actions, obs_out, ref_out, nullptr, nullptr, (cudaStream_t)stream, 0, -1, true, n_steps, 0, references, return_out, end_step_out,
+                 discount, nullptr, &go);
 }
 
 int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, void* obs_out, void* ref_out, void* reward_out,

@@ -17,4 +17,21 @@ struct JacOut {
 
 template <int FAM, typename real> cudaError_t launch_jac_f(bool finite, int nref, const StepParams<real>& p, const JacOut& jo, cudaStream_t st);
 
+// Where the return gradients of gemb200_rollout_return_grads go, and how the reward reads the state row.  ws: the caller's workspace
+// [K][N][W] (W = n_x (n_x + n_u) + n_x + n_u words: one [J_x | J_u | d(g^k r_k)/dx | d(g^k r_k)/da] row per env and step); grad_a [K][N][n_u];
+// grad_x0 [N][n_x]; value_grad [N][n_x] or NULL.  ref_base / rw_base: the entry of the family's state vector (before the wrappers) that
+// reward term r / t reads (StepParams::ref_state / rw_state index the row after the wrappers); wmask: the union of those entries.
+struct GradOut {
+  void* ws;
+  void* grad_a;
+  void* grad_x0;
+  const void* value_grad;
+  int nu;
+  uint32_t wmask;
+  int8_t ref_base[kMaxRef];
+  int8_t rw_base[kMaxState];
+};
+
+template <int FAM, typename real> cudaError_t launch_grad_f(int nref, const StepParams<real>& p, const GradOut& go, cudaStream_t st);
+
 }  // namespace gemb200

@@ -297,28 +297,150 @@ __device__ __forceinline__ int finite_segments(const StepParams<real>& p, const 
   return nseg;
 }
 
-// The tangent pass of one step of env i: writes column c of [jac_x | jac_u] for every seed c
-// into this thread's staging row, jac_x row-major at jrow[r * NX1 + c], jac_u row-major at jrow[NX1 * NX1 + r * nu + c - NX1].
-template <int FAM, bool FINITE, typename real>
-__device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Coef<real>& kc, const real (&x0)[Fam<FAM>::NX], const Ang<real>& ang, const Act<real>& act,
-                                             const unsigned i, const int nu, real* jrow) {
-  using F = Fam<FAM>;
-  constexpr int NX = F::NX, NX1 = NX + (F::EPS ? 1 : 0);
-  const int mech = p.load_kind == GEMB200_LOAD_CONST_SPEED ? 0 : (p.load_kind == GEMB200_LOAD_EXT_SPEED ? 2 : 1);
-  const real rad = rad_per_ang<real>();
-  const real* gt = nullptr;
-  if (mech == 2) {
-    const uint32_t per = 2u * (uint32_t)p.nsteps, last = (uint32_t)p.ext_len - 1u - 2u * per;
-    const uint64_t j0 = (uint64_t)p.kenv[i] * per;
-    gt = p.ext_tab + (j0 < last ? (uint32_t)j0 : last);
-  }
+// The reward-row input of the tangent pass (return_grad_kernel): the step's supply voltage and speed-profile cursor, read before env_step
+// advanced them, and this thread's coefficient row cb[b] = d(g^k r_k) / d s_b over the state-vector entries b in wmask (the weighted ones)
+template <typename real> struct RwTan {
+  real u_sup;
+  const real* gt;
+  const real* cb;
+  uint32_t wmask;
+};
+
+// the supply voltage of the step that starts now (the phase env_step advances afterwards) and this env's speed-profile cursor
+template <typename real> __device__ __forceinline__ real step_u_sup(const StepParams<real>& p, const unsigned i) {
   real u_sup = p.u_sup;
-  if (p.supply_kind == GEMB200_SUPPLY_AC1) {  // the phase at the start of the step (env_step advances it afterwards)
+  if (p.supply_kind == GEMB200_SUPPLY_AC1) {
     Ang<real> ph;
     ph.load(p.sup_phase, i);
     real sph, cph;
     ph.sincos(&sph, &cph);
     u_sup = p.sup_amp * sph;
+  }
+  return u_sup;
+}
+template <typename real> __device__ __forceinline__ const real* step_gt(const StepParams<real>& p, const unsigned i) {
+  if (p.load_kind != GEMB200_LOAD_EXT_SPEED) return nullptr;
+  const uint32_t per = 2u * (uint32_t)p.nsteps, last = (uint32_t)p.ext_len - 1u - 2u * per;
+  const uint64_t j0 = (uint64_t)p.kenv[i] * per;
+  return p.ext_tab + (j0 < last ? (uint32_t)j0 : last);
+}
+
+// v -> rot(-th) v = {c v0 + s v1, -s v0 + c v1} (o: its primal) and its tangent for dv and dth
+template <typename real> __device__ __forceinline__ void rotm_t(real c, real s, const real* v, const real* dv, real dth, real* d) {
+  const real o0 = fm(c, v[0], s * v[1]), o1 = fm(-s, v[0], c * v[1]);
+  d[0] = fm(c, dv[0], s * dv[1]) + dth * o1;
+  d[1] = fm(-s, dv[0], c * dv[1]) - dth * o0;
+}
+
+// Tangent of g^k r_k for one seed column, continuous converters: sum over the weighted entries b of cb[b] * d s_b, s = env_step's state
+// vector after the step (normalised).  x, dx: the state after the step and its tangent; de0, de1: the angle's tangent at the start and
+// the end of the step (rad); dphi: the field angle's (SCIM / DFIM, from the state at the start); du: the converter voltages' tangent;
+// dus: the solver-frame voltages'; us, rab: their primal values (rab: the DFIM's alpha-beta rotor voltages); sn, cs: the rotation of the
+// synchronous motors' currents; snf, csf: the field angle; sne, cse: the DFIM's electrical angle.
+template <int FAM, typename real>
+__device__ __forceinline__ real reward_t(const StepParams<real>& p, const Coef<real>& kc, const RwTan<real>& rw, const real* x, const real* dx, real de0, real de1,
+                                         real dphi, const real* du, const real* dus, const real* us, const real* rab, real sn, real cs, real snf, real csf,
+                                         real sne, real cse) {
+  const uint32_t wm = rw.wmask;
+  const real* cb = rw.cb;
+  real dr = real(0);
+  auto add = [&](int b, real v) { if ((wm >> b) & 1u) dr = fm(cb[b], v * p.inv_lim[b], dr); };
+  auto add_abc = [&](int b, const real* dab) {  // three entries b..b+2 = T32 of an alpha-beta pair
+    if ((wm >> b) & 7u) { real t[3]; t32(dab, t); add(b, t[0]); add(b + 1, t[1]); add(b + 2, t[2]); }
+  };
+  add(0, dx[0]);
+  if constexpr (FAM == kDC1) add(1, (real(2) * kc.tq[1] * x[1] + kc.tq[0]) * dx[1]);
+  else if constexpr (FAM == kDC2) add(1, kc.tq[0] * (dx[1] * x[2] + x[1] * dx[2]));
+  else if constexpr (FAM == kSYNC) add(1, kc.tq[1] * dx[1] * x[2] + (kc.tq[1] * x[1] + kc.tq[0]) * dx[2]);
+  else if constexpr (FAM == kEESM) add(1, (kc.tq[0] * dx[3] + kc.tq[1] * dx[1]) * x[2] + (kc.tq[0] * x[3] + kc.tq[1] * x[1]) * dx[2]);
+  else add(1, kc.tq[0] * (dx[3] * x[2] + x[3] * dx[2] - dx[4] * x[1] - x[4] * dx[1]));
+  const real deps = de1 * (p.eps_out_scale / rad_per_ang<real>());  // the angle entry: inv_lim = 1, scaled by eps_out_scale
+  if constexpr (FAM == kDC1) {
+    add(2, dx[1]); add(3, du[0]);
+  } else if constexpr (FAM == kDC2) {
+    add(2, dx[1]); add(3, dx[2]); add(4, du[0]);
+    if (p.motor_kind == GEMB200_MOTOR_SHUNT_DC) { if ((wm >> 6) & 1u) dr = fm(cb[6], fm(dx[1], p.inv_lim[2], dx[2] * p.inv_lim[3]), dr); }
+    else add(5, du[1]);
+  } else if constexpr (FAM == kSYNC || FAM == kEESM) {
+    // i_abc = T32 q(i_dq, eps at the start of the step)
+    const real ab[2] = {fm(cs, x[1], -(sn * x[2])), fm(sn, x[1], cs * x[2])};
+    const real dab[2] = {fm(cs, dx[1], -(sn * dx[2])) - de0 * ab[1], fm(sn, dx[1], cs * dx[2]) + de0 * ab[0]};
+    add_abc(2, dab);
+    add(5, dx[1]); add(6, dx[2]);
+    if constexpr (FAM == kSYNC) {
+      add(7, du[0]); add(8, du[1]); add(9, du[2]); add(10, dus[0]); add(11, dus[1]);
+      if ((wm >> 12) & 1u) dr = fm(cb[12], deps, dr);
+    } else {
+      add(7, dx[3]); add(8, du[0]); add(9, du[1]); add(10, du[2]); add(11, dus[0]); add(12, dus[1]); add(13, dus[2]);
+      if ((wm >> 14) & 1u) dr = fm(cb[14], deps, dr);
+    }
+  } else {  // SCIM / DFIM: dq quantities in the field frame of the start of the step
+    add_abc(2, dx + 1);
+    real d2[2];
+    rotm_t(csf, snf, x + 1, dx + 1, dphi, d2);
+    add(5, d2[0]); add(6, d2[1]);
+    const real uab[2] = {us[0], us[1]};  // the stator voltages in alpha-beta (the solver frame)
+    real duab[2];
+    t23(du, duab);
+    if constexpr (FAM == kSCIM) {
+      add(7, du[0]); add(8, du[1]); add(9, du[2]);
+      rotm_t(csf, snf, uab, duab, dphi, d2);
+      add(10, d2[0]); add(11, d2[1]);
+      if ((wm >> 12) & 1u) dr = fm(cb[12], deps, dr);
+    } else {
+      // rotor currents (alpha-beta), in the rotor frame (rot(-eps)) and in the field frame (rot(-phi))
+      const real ir[2] = {fm(kc.c[8], x[3], -(kc.c[9] * x[1])), fm(kc.c[8], x[4], -(kc.c[9] * x[2]))};
+      const real dir[2] = {fm(kc.c[8], dx[3], -(kc.c[9] * dx[1])), fm(kc.c[8], dx[4], -(kc.c[9] * dx[2]))};
+      if ((wm >> 7) & 7u) { rotm_t(cse, sne, ir, dir, de0, d2); add_abc(7, d2); }
+      rotm_t(csf, snf, ir, dir, dphi, d2);
+      add(10, d2[0]); add(11, d2[1]);
+      add(12, du[0]); add(13, du[1]); add(14, du[2]);
+      rotm_t(csf, snf, uab, duab, dphi, d2);
+      add(15, d2[0]); add(16, d2[1]);
+      add(17, du[3]); add(18, du[4]); add(19, du[5]);
+      // rotor voltages rot(-(phi - eps)) of their alpha-beta pair
+      const real cfe = fm(csf, cse, snf * sne), sfe = fm(snf, cse, -(csf * sne));
+      real durab[2];
+      t23(du + 3, durab);
+      rotm_t(cfe, sfe, rab, durab, dphi - de0, d2);
+      add(20, d2[0]); add(21, d2[1]);
+      if ((wm >> 22) & 1u) dr = fm(cb[22], deps, dr);
+    }
+  }
+  return dr;
+}
+
+// The tangent pass of one step of env i: writes column c of [jac_x | jac_u] for every seed c
+// into this thread's staging row, jac_x row-major at jrow[r * NX1 + c], jac_u row-major at jrow[NX1 * NX1 + r * nu + c - NX1].
+// RW (continuous converters, return_grad_kernel): also d(g^k r_k) / d(x, a) at jrow[NX1 * (NX1 + nu) + c], from the reward-row input rw;
+// the supply voltage and the speed-profile cursor then come from rw too (the pass runs after env_step, on copies of the pre-step state).
+template <int FAM, bool FINITE, typename real, bool RW = false>
+__device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Coef<real>& kc, const real (&x0)[Fam<FAM>::NX], const Ang<real>& ang, const Act<real>& act,
+                                             const unsigned i, const int nu, real* jrow, const RwTan<real>* rw = nullptr) {
+  static_assert(!(RW && FINITE), "return gradients: continuous converters only");
+  using F = Fam<FAM>;
+  constexpr int NX = F::NX, NX1 = NX + (F::EPS ? 1 : 0);
+  const int mech = p.load_kind == GEMB200_LOAD_CONST_SPEED ? 0 : (p.load_kind == GEMB200_LOAD_EXT_SPEED ? 2 : 1);
+  const real rad = rad_per_ang<real>();
+  const real* gt = nullptr;
+  real u_sup;
+  if constexpr (RW) {
+    gt = rw->gt;
+    u_sup = rw->u_sup;
+  } else {
+    if (mech == 2) {
+      const uint32_t per = 2u * (uint32_t)p.nsteps, last = (uint32_t)p.ext_len - 1u - 2u * per;
+      const uint64_t j0 = (uint64_t)p.kenv[i] * per;
+      gt = p.ext_tab + (j0 < last ? (uint32_t)j0 : last);
+    }
+    u_sup = p.u_sup;
+    if (p.supply_kind == GEMB200_SUPPLY_AC1) {  // the phase at the start of the step (env_step advances it afterwards)
+      Ang<real> ph;
+      ph.load(p.sup_phase, i);
+      real sph, cph;
+      ph.sincos(&sph, &cph);
+      u_sup = p.sup_amp * sph;
+    }
   }
   // ---------------- primal, column-independent: dq rotation of the action, converter voltages and their gains ----------------
   real a[GEMB200_MAX_ACT];
@@ -349,6 +471,7 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
   real usg[MS][4], ubg[MS][4], hsg[MS], kag[MS];
   int nseg = 1;
   real g[6] = {real(0), real(0), real(0), real(0), real(0), real(0)};  // continuous: du_in[l] = g[l] da[l]
+  real rab_p[2] = {real(0), real(0)};  // RW, DFIM: the alpha-beta rotor voltages
   if constexpr (FINITE) {
     nseg = finite_segments<FAM, real>(p, kc, x0, ang, act, i, u_sup, mech, gt, usg, ubg, hsg, kag);
   } else {
@@ -382,6 +505,7 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
         real rab[2];
         t23(u_in + 3, rab);
         us[2] = fm(cse, rab[0], -(sne * rab[1])); us[3] = fm(sne, rab[0], cse * rab[1]);
+        if constexpr (RW) { rab_p[0] = rab[0]; rab_p[1] = rab[1]; }
       }
     } else {
 #pragma unroll
@@ -400,6 +524,11 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
     kag[0] = F::EPS ? p.kang[mech ? 1 : 0][0][0] * rad : real(0);  // d eps (rad) / d wsum
   }
   const real adv = p.adv_k * rad;
+  real snf = real(0), csf = real(1), r2p = real(0);  // RW, SCIM / DFIM: the field angle at the start of the step
+  if constexpr (RW && (FAM == kSCIM || FAM == kDFIM)) {
+    r2p = fm(x0[3], x0[3], x0[4] * x0[4]);
+    if (r2p > real(0)) { const real ir = Num<real>::rsqrt(r2p); csf = x0[3] * ir; snf = x0[4] * ir; }
+  }
   // ---------------- one tangent pass per seed column ----------------
   const int ncol = NX1 + nu;
 #pragma unroll 1
@@ -408,6 +537,9 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
 #pragma unroll
     for (int j = 0; j < NX; ++j) { x[j] = x0[j]; dx[j] = c == j ? real(1) : real(0); }
     real de = (F::EPS && c == NX) ? real(1) : real(0);  // tangent of the angle (rad), seeded in its own column
+    const real de0 = de;
+    real dphi = real(0);  // RW: the field angle's tangent
+    if constexpr (RW && (FAM == kSCIM || FAM == kDFIM)) dphi = r2p > real(0) ? (x0[3] * dx[4] - x0[4] * dx[3]) / r2p : real(0);
     real da[GEMB200_MAX_ACT];
 #pragma unroll
     for (int j = 0; j < GEMB200_MAX_ACT; ++j) da[j] = c - NX1 == j ? real(1) : real(0);
@@ -424,10 +556,15 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
     }
     // continuous converters: the action part of the voltages (one segment); finite converters have none
     real dab[2] = {real(0), real(0)}, drab[2] = {real(0), real(0)}, dq3[2] = {real(0), real(0)};
+    real dui[6], dus0[4];  // RW: the converter and solver-frame voltages' tangents
     if constexpr (!FINITE) {
       real du[6];
 #pragma unroll
       for (int l = 0; l < 6; ++l) du[l] = g[l] * da[l];
+      if constexpr (RW) {
+#pragma unroll
+        for (int l = 0; l < 6; ++l) dui[l] = du[l];
+      }
       if constexpr (FAM == kSYNC || FAM == kEESM || FAM == kSCIM || FAM == kDFIM) {
         t23(du, dab);
         if constexpr (FAM == kEESM) dq3[0] = du[3];
@@ -450,6 +587,10 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
       if constexpr (FAM == kDFIM) {  // rotor voltages rotated by +eps
         dus[2] = fm(cse, drab[0], -(sne * drab[1])) - de * us[3]; dus[3] = fm(sne, drab[0], cse * drab[1]) + de * us[2];
       }
+      if constexpr (RW) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) dus0[j] = dus[j];
+      }
       real dub[4];
       Model<FAM, real>::ubias(kc, dus, dub);
       dws = integrate_t<FAM, real>(p, kc, x, dx, ubg[seg], dub, hsg[seg], mech, gt);
@@ -465,6 +606,8 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
       for (int r = 0; r < NX; ++r) ju[r * nu] = dx[r];
       if constexpr (F::EPS) ju[NX * nu] = de;
     }
+    if constexpr (RW)
+      jrow[NX1 * (NX1 + nu) + c] = reward_t<FAM, real>(p, kc, *rw, x, dx, de0, de, dphi, dui, dus0, usg[0], rab_p, sn, cs, snf, csf, sne, cse);
   }
 }
 
@@ -575,6 +718,212 @@ jacobian_kernel(const __grid_constant__ StepParams<real> p, const __grid_constan
     if constexpr (NH > 0) store_words<NH, real>(p.st, i, n, hot);
     if (cold_dirty) store_words<NC, real>(p.stc, i, n, cold);
     if constexpr (F::EPS) ang.store(p.eps, i);
+  }
+}
+
+// The load counterpart of warp_store_jac: the warp's rows (width w words) from `src` (the warp's first env's row) into shared memory
+template <typename real>
+__device__ __forceinline__ void warp_load_jac(real* __restrict__ rows, const real* __restrict__ src, int stride, int w, int valid, int lane) {
+  const int total = valid * w;
+#pragma unroll 1
+  for (int k = lane; k < total; k += 32) { const int e = k / w; rows[e * stride + (k - e * w)] = src[k]; }
+}
+
+// A reward term's derivative with respect to its row entry: r = bias - sum w |(row - ref) inv_len|^pw, so d r / d row =
+// -w pw |e inv_len|^(pw - 1) sgn(e) inv_len with e = row - ref, taken as 0 at e = 0 (the one-sided convention of DESIGN.md §7)
+template <typename real>
+__device__ __forceinline__ real reward_coef(real e, real inv_len, real w, int pow1, real pw) {
+  const real ae = Num<real>::abs(e) * inv_len;
+  real d = sgn(e) * inv_len;
+  if (!pow1) d = ae > real(0) ? d * (pw * Num<real>::pow(ae, pw - real(1))) : real(0);
+  return -(w * d);
+}
+
+// The K-step loop of return_grad_kernel: rollout_loop's discounted return (same updates, same roundings), the tangent pass of every step
+// up to the env's first termination with its row [J_x | J_u | d(g^k r_k)/dx | d(g^k r_k)/da] stored to the workspace, then the reverse
+// sweep over those rows:  lambda = g^K value_grad (no termination) or 0;  for k = min(end, K) - 1 .. 0:  grad_a[k] = d(g^k r_k)/da +
+// J_u^T lambda,  lambda = d(g^k r_k)/dx + J_x^T lambda;  grad_x0 = lambda.
+template <int FAM, typename real, int NREF, bool ENVP>
+__device__ __forceinline__ RetAcc<real> grad_loop(const StepParams<real>& p, const GradOut& go, CoefArg<real, ENVP> kc, const unsigned i, const bool active,
+                                                  real (&x)[Fam<FAM>::NX], Ang<real>& ang, real (&rv)[NREF > 0 ? NREF : 1], real (&rs)[NREF > 0 ? NREF : 1],
+                                                  uint32_t (&rend)[NREF > 0 ? NREF : 1], bool& cold_dirty, real* rows, real* row, real* jrows, real* jrow,
+                                                  const int jstride, const int lane, const int stride) {
+  using F = Fam<FAM>;
+  constexpr int NX = F::NX, NX1 = NX + (F::EPS ? 1 : 0), NS = F::NS;
+  const int K = p.roll_steps;
+  const int nu = go.nu;
+  const int W = NX1 * (NX1 + nu) + NX1 + nu;
+  const size_t n = (size_t)(unsigned)p.n;
+  Out<real> out = make_out<NREF, false, real>(p, i, lane, p.n_obs);
+  ClockArg<ENVP> ck = clock_of(p);
+  if constexpr (ENVP) ck = id_clock(p, clock_of(p), active ? i : (unsigned)p.env_begin);
+  const char* act = action_cursor<FAM, false, real, false>(p, p.action, i);
+  WalkCache wc{};
+  Act<real> a_next{};
+  if (active) a_next = load_action<FAM, false, real, false>(p, act);
+  constexpr bool kFeed = NREF > 0;
+  const bool feed = kFeed && p.ref_feed != nullptr;
+  const real* fc = nullptr;
+  real f_next[NREF > 0 ? NREF : 1];
+  if constexpr (kFeed) {
+    if (feed) { fc = feed_cursor<NREF, false, real>(p, i); if (active) load_feed<NREF, false, real>(p, fc, f_next); }
+  }
+  const size_t warp_env0 = i - lane;
+  real* ws = static_cast<real*>(go.ws) + warp_env0 * (size_t)W;
+  real* cb = jrow + W;  // the coefficient row of the reward tangent, behind the stash row
+  RetAcc<real> acc{real(0), K};
+  real w = real(1);
+#pragma unroll 1
+  for (int k = 0; k < K; ++k) {
+    const Act<real> a_cur = a_next;
+    act += p.roll_act_inc;
+    if (active && k + 1 < K) a_next = load_action<FAM, false, real, false>(p, act);
+    if constexpr (kFeed) {
+      if (feed) {
+#pragma unroll
+        for (int r = 0; r < NREF; ++r) rv[r] = f_next[r];
+        fc += n * NREF;
+        if (active && k + 1 < K) load_feed<NREF, false, real>(p, fc, f_next);
+      }
+    }
+    // what the tangent pass reads and env_step advances: the state, the angle, the references the reward compares with, the supply
+    // voltage and the speed-profile cursor of this step
+    const bool alive = active && acc.end == K;
+    real x0[NX], rv0[NREF > 0 ? NREF : 1];
+#pragma unroll
+    for (int j = 0; j < NX; ++j) x0[j] = x[j];
+#pragma unroll
+    for (int r = 0; r < (NREF > 0 ? NREF : 1); ++r) rv0[r] = rv[r];
+    const Ang<real> ang0 = ang;
+    RwTan<real> rt{real(0), nullptr, cb, go.wmask};
+    if (alive) { rt.u_sup = step_u_sup(p, i); rt.gt = step_gt(p, i); }
+    const StepOut<real> so = env_step<FAM, false, real, NREF, false, false, false, false, ENVP>(p, kc, ck, out, k == K - 1, a_cur, i, active, x, ang, rv, rs, rend,
+                                                                                               cold_dirty, wc, rows, row, lane, stride);
+    if (alive) {
+      acc.g = acc.g + w * so.reward;
+      if (so.term) acc.end = k;
+    }
+    const bool lin = alive && !so.term;  // a step whose row the sweep reads
+    if (lin) {  // d(w r_k) / d s_b from the row env_step left (state noise included), then the tangent pass on the pre-step copies
+#pragma unroll
+      for (int b = 0; b < NS; ++b) if ((go.wmask >> b) & 1u) cb[b] = real(0);
+#pragma unroll
+      for (int r = 0; r < NREF; ++r)
+        if (p.rwr_w[r] != real(0)) cb[go.ref_base[r]] += w * reward_coef(row[p.ref_state[r]] - rv0[r], p.rwr_inv_len[r], p.rwr_w[r], p.rwr_pow1[r], p.rwr_pow[r]);
+#pragma unroll 1
+      for (int t = 0; t < p.n_rw; ++t)
+        cb[go.rw_base[t]] += w * reward_coef(row[p.rw_state[t]], p.rw_inv_len[t], p.rw_w[t], p.rw_pow1[t], p.rw_pow[t]);
+      step_tangent<FAM, false, real, true>(p, kc, x0, ang0, a_cur, i, nu, jrow, &rt);
+    }
+    w = w * p.discount;
+    __syncwarp();
+    if (__any_sync(0xffffffffu, lin)) warp_store_jac(ws, jrows, jstride, W, out.valid, lane);
+    ws += n * (size_t)W;
+    __syncwarp();  // both staging areas are reused by the next step
+    ck.kstep += 1u;
+    ck.gstep_lo += 1u;
+    if (ck.gstep_lo == 0u) ck.gstep_hi += 1u;
+  }
+  // ---------------- reverse sweep ----------------
+  real lam[NX1];
+  const bool boot = active && acc.end == K && go.value_grad != nullptr;
+#pragma unroll
+  for (int r = 0; r < NX1; ++r) lam[r] = boot ? w * static_cast<const real*>(go.value_grad)[(size_t)i * NX1 + r] : real(0);
+  real* ga_out = static_cast<real*>(go.grad_a) + (size_t)K * n * nu + warp_env0 * (size_t)nu;
+#pragma unroll 1
+  for (int k = K - 1; k >= 0; --k) {
+    ws -= n * (size_t)W;
+    ga_out -= n * (size_t)nu;
+    const bool live = active && k < acc.end;
+    if (__any_sync(0xffffffffu, live)) warp_load_jac(jrows, ws, jstride, W, out.valid, lane);
+    __syncwarp();
+    real ga[GEMB200_MAX_ACT];
+    const real* jx = jrow;
+    const real* ju = jrow + NX1 * NX1;
+    const real* rx = jrow + NX1 * (NX1 + nu);
+    const real* ru = rx + NX1;
+#pragma unroll
+    for (int u = 0; u < GEMB200_MAX_ACT; ++u) {
+      real s = real(0);
+      if (live && u < nu) {
+        s = ru[u];
+#pragma unroll
+        for (int r = 0; r < NX1; ++r) s = fm(ju[r * nu + u], lam[r], s);
+      }
+      ga[u] = s;
+    }
+    if (live) {
+      real ln[NX1];
+#pragma unroll
+      for (int c = 0; c < NX1; ++c) {
+        real s = rx[c];
+#pragma unroll
+        for (int r = 0; r < NX1; ++r) s = fm(jx[r * NX1 + c], lam[r], s);
+        ln[c] = s;
+      }
+#pragma unroll
+      for (int c = 0; c < NX1; ++c) lam[c] = ln[c];
+    }
+    __syncwarp();
+#pragma unroll
+    for (int u = 0; u < GEMB200_MAX_ACT; ++u) if (u < nu) jrow[u] = ga[u];
+    __syncwarp();
+    warp_store_jac(ga_out, jrows, jstride, nu, out.valid, lane);
+    __syncwarp();
+  }
+#pragma unroll
+  for (int c = 0; c < NX1; ++c) jrow[c] = lam[c];
+  __syncwarp();
+  warp_store_jac(static_cast<real*>(go.grad_x0) + warp_env0 * NX1, jrows, jstride, NX1, out.valid, lane);
+  return acc;
+}
+
+// The return-gradient kernel (continuous converters): jacobian_kernel's shape with grad_loop, and rollout_kernel's returns.  Dynamic shared
+// memory: the observation rows of the block, then per env its stash row and its coefficient row (jstride words).
+template <int FAM, typename real, int NREF, bool ENVP>
+__global__ void __launch_bounds__(GEMB200_BLOCK, (sizeof(real) == 4 ? GEMB200_MINBLOCKS_JAC : GEMB200_MINBLOCKS_JAC_F64))
+return_grad_kernel(const __grid_constant__ StepParams<real> p, const __grid_constant__ GradOut go, const int jstride) {
+  using F = Fam<FAM>;
+  constexpr int NX = F::NX, NH = hot_words(NX, NREF), NC = cold_words(NX, NREF);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  real* smem = reinterpret_cast<real*>(smem_raw);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int stride = p.row_stride;
+  real* rows = smem + warp * (32 * stride);
+  real* row = rows + lane * stride;
+  real* jrows = smem + blockDim.x * stride + warp * (32 * jstride);
+  real* jrow = jrows + lane * jstride;
+  const unsigned i = (unsigned)p.env_begin + blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned n = (unsigned)p.n;
+  const bool active = i < (unsigned)p.env_end;
+  const int mech = p.load_kind != GEMB200_LOAD_CONST_SPEED;
+  real hot[NH > 0 ? NH : 1], cold[NC];
+  Ang<real> ang;
+  real x[NX], rv[NREF > 0 ? NREF : 1], rs[NREF > 0 ? NREF : 1];
+  uint32_t rend[NREF > 0 ? NREF : 1];
+  bool cold_dirty = mech;
+  if (active) {
+    if constexpr (NH > 0) load_words<NH, real>(p.st, i, n, hot);
+    load_words<NC, real>(p.stc, i, n, cold);
+    ang.set(p.init_ang);
+    if constexpr (F::EPS) ang.load(p.eps, i);
+    unpack_records<NX, NREF, real>(hot, cold, x, rv, rs, rend);
+  }
+  RetAcc<real> acc;
+  if constexpr (ENVP) {
+    Coef<real> kl;
+    load_coef<FAM, real>(p, active ? i : (unsigned)p.env_begin, mech != 0, kl);
+    acc = grad_loop<FAM, real, NREF, true>(p, go, kl, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
+  } else {
+    acc = grad_loop<FAM, real, NREF, false>(p, go, p.k, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
+  }
+  if (active) {
+    pack_records<NX, NREF, real>(hot, cold, x, rv, rs, rend);
+    if constexpr (NH > 0) store_words<NH, real>(p.st, i, n, hot);
+    if (cold_dirty) store_words<NC, real>(p.stc, i, n, cold);
+    if constexpr (F::EPS) ang.store(p.eps, i);
+    p.ret_out[i] = acc.g;
+    if (p.ret_end) p.ret_end[i] = acc.end;
   }
 }
 

@@ -346,6 +346,61 @@ class VectorSim:
                                                     _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term), self._stream()),
                 "gemb200_rollout_jacobians")
 
+    def return_grad_dims(self):
+        """(n_x, n_u, ws_words) of `rollout_return_grads`: n_x = n_ode, n_u = n_act, ws_words = n_x (n_x + n_u) + n_x + n_u, the workspace
+        words per env and step.  NotImplementedError for a configuration the launch refuses (DESIGN.md §7)."""
+        lib = K.load_library()  # a configuration query: no handle, no launch
+        nx, nu, ww = C.c_int32(), C.c_int32(), C.c_int32()
+        if lib.gemb200_query_return_grad_dims(C.byref(self.cfg), C.byref(nx), C.byref(nu), C.byref(ww)):
+            raise NotImplementedError(lib.gemb200_last_error().decode())
+        return nx.value, nu.value, ww.value
+
+    def _as_value_grad(self, value_grad, nx):
+        if value_grad is None:
+            return None
+        shape = (self.n, nx)
+        if (not isinstance(value_grad, torch.Tensor) or value_grad.dtype != self.dtype or value_grad.device != self.device
+                or tuple(value_grad.shape) != shape or not value_grad.is_contiguous()):
+            got = (f"{tuple(value_grad.shape)} {value_grad.dtype} on {value_grad.device}" if isinstance(value_grad, torch.Tensor)
+                   else type(value_grad).__name__)
+            raise ValueError(f"value_grad must be a contiguous [{self.n}, {nx}] {self.dtype} tensor on {self.device}, got {got}")
+        return value_grad
+
+    def rollout_return_grads(self, actions, discount=1.0, references=None, value_grad=None):
+        """`rollout_returns` with the gradients of the returns (gemb200_rollout_return_grads), in ONE launch.  Returns (returns, end_step,
+        (obs, ref), grad_a, grad_x0): the first three exactly as `rollout_returns(actions, discount, references)` returns them (and the
+        same final state, clock and RNG position); grad_a [K, N, n_u] = d returns[i] / d a_k[i] for the caller's action, 0 for
+        k >= end_step[i]; grad_x0 [N, n_x] = d returns[i] / d x_0[i], x the ODE state of `get_ode_state` (the angle last, in radians).
+        value_grad [N, n_x] (handle dtype) adds discount^K value_grad[i] to the adjoint of every env with end_step == K.  The workspace,
+        K * N * ws_words words, is a torch allocation of this call.  Refused configurations: NotImplementedError (DESIGN.md §7); bad
+        actions, discount, feed or value_grad: ValueError before any launch."""
+        nx, nu, ww = self.return_grad_dims()
+        a = self._as_actions(actions)
+        k = int(a.shape[0])
+        g = self._as_discount(discount)
+        r = None if references is None else self._as_feed(references, k)
+        vg = self._as_value_grad(value_grad, nx)
+        obs, ref, _, _ = self._alloc_outputs()
+        ret = torch.empty(self.n, dtype=self.dtype, device=self.device)
+        end = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        ga = torch.empty((k, self.n, nu), dtype=self.dtype, device=self.device)
+        gx = torch.empty((self.n, nx), dtype=self.dtype, device=self.device)
+        ws = torch.empty(k * self.n * ww, dtype=self.dtype, device=self.device)
+        self.rollout_return_grads_into(a, k, g, ws, ret, end, ga, gx, obs, ref, r, vg)
+        return ret, end, (obs, ref), ga, gx
+
+    def rollout_return_grads_into(self, actions, n_steps, discount, workspace, ret, end, grad_a, grad_x0, obs=None, ref=None, references=None,
+                                  value_grad=None):
+        """Raw variant of `rollout_return_grads` for benchmarking: caller-owned outputs and workspace (a device tensor of at least
+        n_steps * N * ws_words elements of the handle's dtype; `end`, `obs`, `ref` and `value_grad` may be None), no allocation, no
+        conversion.  The discount and the reference feed are checked like there."""
+        g = self._as_discount(discount)
+        r = None if references is None else self._as_feed(references, n_steps)
+        K.check(self._lib.gemb200_rollout_return_grads(self._h, _ptr(actions), _ptr(r), int(n_steps), g, _ptr(value_grad), _ptr(workspace),
+                                                       workspace.numel() * workspace.element_size(), _ptr(ret), _ptr(end), _ptr(grad_a),
+                                                       _ptr(grad_x0), _ptr(obs), _ptr(ref) if self.n_ref else None, self._stream()),
+                "gemb200_rollout_return_grads")
+
     # ------------------------------------------------------------------ host-buffer API (numpy)
     def step_host(self, action, out=None):
         """Same step through HOST buffers (the C-ABI does H2D, launch, D2H, sync).  `out` = tuple of numpy arrays to

@@ -352,6 +352,23 @@ int gemb200_query_jacobian_dims(const gemb200_config* cfg, int32_t* n_x, int32_t
 int gemb200_rollout_jacobians(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, void* jac_x_out, void* jac_u_out,
                               void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream);
 
+/* Gradients of rollout returns (continuous converters).  gemb200_query_return_grad_dims (needs no GPU): n_x = n_ode and n_u = n_act as for
+ * the Jacobians, ws_words = n_x (n_x + n_u) + n_x + n_u; refuses everything gemb200_query_jacobian_dims refuses, finite converters, and a
+ * reward that weights an entry a state wrapper appends (GEMB200_E_INVALID, DESIGN.md §7).
+ * gemb200_rollout_return_grads: n_steps = K open-loop steps in ONE launch.  return_out [N], end_step_out [N] (may be NULL), obs_out and
+ * ref_out (may be NULL) are exactly what gemb200_rollout_returns(actions, references, K, discount) writes, and the final state, clock and
+ * RNG position are those of that call.  Per env i with e = end_step[i]:
+ *   grad_a_out [K][N][n_u] = d return[i] / d a_k[i] (the caller's action, dq under action_dq = 1), 0 for k >= e;
+ *   grad_x0_out [N][n_x]   = d return[i] / d x_0[i] (x as gemb200_get_ode_state: the angle last, in radians), 0 when e == 0.
+ * value_grad [N][n_x] (or NULL) adds gamma^K value_grad[i] to the adjoint of every env with e == K (return_out is unchanged).  Non-smooth
+ * points take the one-sided derivative of the branch the step took, and termination has derivative 0.  workspace: the caller's work buffer of at
+ * least K * N * ws_words * sizeof(real) bytes (one linearised step per env and step); the call allocates nothing.  All buffers are device
+ * memory in the handle's dtype, row-per-env.  Stream-ordered, capturable in a CUDA graph under the device clock. */
+int gemb200_query_return_grad_dims(const gemb200_config* cfg, int32_t* n_x, int32_t* n_u, int32_t* ws_words);
+int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, double discount, const void* value_grad,
+                                 void* workspace, uint64_t workspace_bytes, void* return_out, int32_t* end_step_out, void* grad_a_out, void* grad_x0_out,
+                                 void* obs_out, void* ref_out, void* stream);
+
 /* OdeSolver.y / set_initial_value (physical_systems/solvers.py:4-76): ODE state as double [N][n_ode]
  * (AoS, device), angle unwrapped to (-pi, pi].  Used for checkpointing and oracle injection. */
 int gemb200_get_ode_state(gemb200_handle* h, double* ode_out, void* stream);
