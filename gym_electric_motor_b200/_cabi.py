@@ -148,7 +148,8 @@ SYMBOLS = [
     "gemb200_version", "gemb200_last_error", "gemb200_config_init", "gemb200_query_dims", "gemb200_create",
     "gemb200_destroy", "gemb200_reset", "gemb200_step", "gemb200_step_host", "gemb200_reset_host", "gemb200_rollout", "gemb200_rollout_record",
     "gemb200_rollout_record_ref", "gemb200_rollout_returns", "gemb200_query_jacobian_dims", "gemb200_rollout_jacobians",
-    "gemb200_query_return_grad_dims", "gemb200_rollout_return_grads",
+    "gemb200_query_return_grad_dims", "gemb200_rollout_return_grads", "gemb200_query_param_sens_dims", "gemb200_coef_tangents",
+    "gemb200_rollout_param_sens",
     "gemb200_get_ode_state", "gemb200_set_ode_state", "gemb200_get_reference", "gemb200_set_reference",
     "gemb200_reseed", "gemb200_set_device_clock", "gemb200_get_clock", "gemb200_set_env_params", "gemb200_peer_buffer_alloc", "gemb200_peer_buffer_open", "gemb200_peer_buffer_close",
     "gemb200_peer_buffer_free", "gemb200_bind_peers", "gemb200_peer_signal", "gemb200_peer_wait", "gemb200_checkpoint_size", "gemb200_checkpoint_save", "gemb200_checkpoint_load", "gemb200_query_env_record",
@@ -202,6 +203,9 @@ def load_library():
     lib.gemb200_rollout_jacobians.argtypes = [vp, vp, vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
     lib.gemb200_query_return_grad_dims.argtypes = [cfgp, i32p, i32p, i32p]
     lib.gemb200_rollout_return_grads.argtypes = [vp, vp, vp, C.c_int32, C.c_double, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, vp]
+    lib.gemb200_query_param_sens_dims.argtypes = [cfgp, C.c_int32, i32p, i32p]
+    lib.gemb200_coef_tangents.argtypes = [cfgp, vp, vp, C.c_int32, i32p, vp]
+    lib.gemb200_rollout_param_sens.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, i32p, vp, vp, vp, vp, vp, vp, vp]
     lib.gemb200_get_ode_state.argtypes = [vp, vp, vp]
     lib.gemb200_set_ode_state.argtypes = [vp, vp, vp]
     lib.gemb200_get_reference.argtypes = [vp, vp, vp]

@@ -372,6 +372,55 @@ class ElectricMotorEnvironment(_EnvBase):
             raise ValueError(f"actions must be a torch tensor, got {type(actions).__name__}")
         return _DifferentiableReturns.apply(actions, self, discount, references)
 
+    def param_slots(self, params):
+        """The parameter-row slots of the names `params` (the names of `set_env_parameters`): KeyError for an unknown name, ValueError for
+        the pole pairs `p`, the EESM's `k` (DESIGN.md §7), an empty list or a parameter named twice (`r_r` is `r_e`)."""
+        if isinstance(params, str):
+            params = [params]
+        slots = []
+        for name in params:
+            if name in self._MP_SLOT:
+                if name in ("p", "k"):
+                    raise ValueError(f"parameter sensitivities with respect to {name!r} are not provided: "
+                                     + ("the angle increments are prepared per env handle" if name == "p" else "the EESM's coefficients are invariant in k")
+                                     + " (DESIGN.md §7)")
+                slot = self._MP_SLOT[name]
+            elif name in self._LP_SLOT:
+                slot = K.MAX_MOTOR_PARAM + self._LP_SLOT[name]
+            else:
+                raise KeyError(f"unknown parameter {name!r}")
+            if slot in slots:
+                raise ValueError(f"parameter {name!r} is named twice")
+            slots.append(slot)
+        if not 1 <= len(slots) <= 12:
+            raise ValueError(f"parameter sensitivities take 1 to 12 parameters, got {len(slots)}")
+        return slots
+
+    def rollout_param_sensitivities(self, actions, params, references=None, sens0=None, record=True):
+        """Parameter sensitivities along an action sequence: K steps with pre-computed actions [K, N, n_act] in ONE kernel launch that also
+        carries, per env i, S = d x / d theta[i] with respect to the env's OWN physical parameters `params` (a list of the names
+        `set_env_parameters` takes; `p` and `k` are refused).  x is the ODE state of `get_ode_state` (the angle last, in radians).  Returns
+        ((sens, sens_last), ((states, references), rewards, terminateds)): sens [K, N, n_x, n_p] = d x_{k+1} / d theta after every step
+        (None when record=False), sens_last [N, n_x, n_p] the carried S after the last step, to pass as `sens0` of the next call; the second
+        part exactly as `rollout(actions, record_every=1, references=references)` returns it, and the env ends in that call's state.  sens0:
+        S at the start (None: zeros, the sensitivity of the trajectory from the current state).  A terminating step reports the sensitivity
+        of the physical step it took; an env auto-reset in it carries S = 0 from there.  Refused configurations (those of
+        `rollout_jacobians`) and parameter draws at resets: NotImplementedError (DESIGN.md §7).  Batched mode only; bad actions, feed or
+        sens0: ValueError before any launch."""
+        if self._scalar:
+            raise TypeError("rollout_param_sensitivities() needs a batched environment (num_envs=...)")
+        slots = self.param_slots(params)
+        sim = self._ensure_sim()
+        if getattr(self, "_randomized_names", ()):
+            raise NotImplementedError("parameter sensitivities are refused while parameter draws at resets are on (DESIGN.md §7)")
+        (so, sl), (obs, ref, reward, terminated) = sim.rollout_param_sens(actions, slots, references, sens0, record)
+        self._physical_system._k += int(actions.shape[0])
+        if not self._filter_identity:
+            if self._filter_index is None:
+                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
+            obs = obs.index_select(2, self._filter_index)
+        return (so, sl), ((obs, ref), reward, terminated.view(torch.bool))
+
     def capture_steps(self, policy, n_steps, record=False, warmup=1, references=None):
         """`n_steps` closed-loop steps — action = policy(state, reference); env.step(action) — captured ONCE in a CUDA graph (graph.py);
         `.replay()` of the returned object runs them with a single call.  Batched mode only.  references: a static reference feed

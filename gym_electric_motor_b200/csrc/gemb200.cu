@@ -694,6 +694,23 @@ static cudaError_t launch_grad(int fam, int nref, const StepParams<real>& p, con
 }
 
 template <typename real>
+static cudaError_t launch_psens(int fam, bool finite, int nref, const StepParams<real>& p, const PsOut& po, cudaStream_t st) {
+#ifdef GEMB200_ONLY_FAM
+  return cudaErrorInvalidValue;
+#else
+  switch (fam) {
+    case kDC1: return launch_psens_f<kDC1, real>(finite, nref, p, po, st);
+    case kDC2: return launch_psens_f<kDC2, real>(finite, nref, p, po, st);
+    case kSYNC: return launch_psens_f<kSYNC, real>(finite, nref, p, po, st);
+    case kEESM: return launch_psens_f<kEESM, real>(finite, nref, p, po, st);
+    case kSCIM: return launch_psens_f<kSCIM, real>(finite, nref, p, po, st);
+    case kDFIM: return launch_psens_f<kDFIM, real>(finite, nref, p, po, st);
+  }
+  return cudaErrorInvalidValue;
+#endif
+}
+
+template <typename real>
 static void set_roll_strides(const gemb200_handle* h, StepParams<real>& p) {
   const int64_t n = h->cfg.n_envs;
   p.out_has = (p.obs ? 1 : 0) | ((p.ref_out && h->n_ref > 0) ? 2 : 0) | (p.reward ? 4 : 0) | (p.term ? 8 : 0);
@@ -739,10 +756,12 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
 // feed: the reference values of every step (StepParams::ref_feed), or NULL.  ret / ret_end / discount: the discounted returns of a
 // rollout (StepParams::ret_out), or NULL.  jac: the Jacobian outputs of gemb200_rollout_jacobians, or NULL; with them the launch takes the
 // rollout-Jacobian kernel (gemb200_tangent.cuh) instead of the step / rollout kernels.  grad: the outputs of gemb200_rollout_return_grads,
-// or NULL; with them the launch takes the return-gradient kernel (gemb200_tangent.cuh).
+// or NULL; with them the launch takes the return-gradient kernel (gemb200_tangent.cuh).  ps: the parameter-sensitivity outputs of
+// gemb200_rollout_param_sens, or NULL; with them the launch takes the parameter-sensitivity kernel (gemb200_tangent.cuh).
 static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, void* rew, uint8_t* term, cudaStream_t st,
                    int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr,
-                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const JacOut* jac = nullptr, const GradOut* grad = nullptr) {
+                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const JacOut* jac = nullptr, const GradOut* grad = nullptr,
+                   const PsOut* ps = nullptr) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
@@ -763,6 +782,7 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     set_roll_strides(h, p);
     if (jac) return launch_jac<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, *jac, st);
     if (grad) return launch_grad<real>(h->fam, h->n_ref, p, *grad, st);
+    if (ps) return launch_psens<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, *ps, st);
     return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
   });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string(roll > 0 ? "rollout launch: " : "step launch: ") + cudaGetErrorString(e));
@@ -925,6 +945,50 @@ int gemb200_query_return_grad_dims(const gemb200_config* cfg, int32_t* n_x, int3
   if (n_x) *n_x = d.n_ode;
   if (n_u) *n_u = d.n_act;
   if (ws_words) *ws_words = d.n_ode * (d.n_ode + d.n_act) + d.n_ode + d.n_act;
+  return GEMB200_OK;
+}
+
+// Parameter sensitivities (DESIGN.md §7, "Parameter sensitivities"): the reason a configuration or a list of parameter slots is refused,
+// or nullptr.  Accepted: every motor slot but the pole pairs and the EESM's k, and the load slots a, b, c, j_load.
+static const char* param_sens_refusal(const gemb200_config* c, int32_t n_p, const int32_t* slots) {
+  if (const char* why = jacobian_refusal(c)) return why;
+  if (n_p < 1 || n_p > kMaxSensParams) return "parameter sensitivities: n_p must be in [1, 12] (DESIGN.md §7)";
+  if (!slots) return "parameter sensitivities: slots is NULL";
+  for (int a = 0; a < n_p; ++a) {
+    const int s = slots[a];
+    const bool motor = s >= 0 && s < GEMB200_MAX_MOTOR_PARAM;
+    const int l = s - GEMB200_MAX_MOTOR_PARAM;
+    if (!motor && !(l == GEMB200_LP_A || l == GEMB200_LP_B || l == GEMB200_LP_C || l == GEMB200_LP_J_LOAD))
+      return "parameter sensitivities: a slot is neither a motor slot nor one of the load slots a, b, c, j_load (DESIGN.md §7)";
+    if (s == GEMB200_MP_P) return "parameter sensitivities: the pole pairs are refused, the angle increments are prepared per handle (DESIGN.md §7)";
+    if (s == GEMB200_MP_K) return "parameter sensitivities: the EESM's k is refused, the model coefficients are invariant in it (DESIGN.md §7)";
+    for (int b = 0; b < a; ++b)
+      if (slots[b] == s) return "parameter sensitivities: duplicate slot (DESIGN.md §7)";
+  }
+  return nullptr;
+}
+
+int gemb200_query_param_sens_dims(const gemb200_config* cfg, int32_t n_p, const int32_t* slots, int32_t* n_x) {
+  if (!cfg) return fail(GEMB200_E_INVALID, "config is NULL");
+  Dims d;
+  int rc = derive_dims(cfg, &d);
+  if (rc) return rc;
+  if (const char* why = param_sens_refusal(cfg, n_p, slots)) return fail(GEMB200_E_INVALID, why);
+  if (n_x) *n_x = d.n_ode;
+  return GEMB200_OK;
+}
+
+int gemb200_coef_tangents(const gemb200_config* cfg, const double* motor_param, const double* load_param, int32_t n_p, const int32_t* slots, double* out) {
+  if (!cfg) return fail(GEMB200_E_INVALID, "config is NULL");
+  if (!out) return fail(GEMB200_E_INVALID, "out is NULL");
+  Dims d;
+  int rc = derive_dims(cfg, &d);
+  if (rc) return rc;
+  if (const char* why = param_sens_refusal(cfg, n_p, slots)) return fail(GEMB200_E_INVALID, why);
+  double prm[kMaxDraw];
+  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) prm[s] = motor_param ? motor_param[s] : cfg->motor_param[s];
+  for (int s = 0; s < 8; ++s) prm[GEMB200_MAX_MOTOR_PARAM + s] = load_param ? load_param[s] : cfg->load_param[s];
+  for (int a = 0; a < n_p; ++a) coef_tangent(cfg->motor_kind, prm, slots[a], out + (size_t)a * kCoefWords);
   return GEMB200_OK;
 }
 
@@ -1102,6 +1166,25 @@ int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const v
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, nullptr, nullptr, (cudaStream_t)stream, 0, -1, true, n_steps, 0, references, return_out, end_step_out,
                  discount, nullptr, &go);
+}
+
+int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t n_p, const int32_t* slots,
+                               void* sens_io, void* sens_out, void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  if (const char* why = param_sens_refusal(&h->cfg, n_p, slots)) return fail(GEMB200_E_INVALID, why);
+  if (draws_on(h))
+    return fail(GEMB200_E_INVALID, "parameter sensitivities: parameter draws at resets are on, the parameters would change inside the launch (DESIGN.md §7)");
+  if (!sens_io) return fail(GEMB200_E_INVALID, "sens_io is NULL");
+  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
+  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  PsOut po{};
+  po.sio = sens_io; po.sout = sens_out; po.np = n_p;
+  for (int a = 0; a < n_p; ++a) po.slot[a] = slots[a];
+  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) po.raw[s] = h->cfg.motor_param[s];
+  for (int s = 0; s < 8; ++s) po.raw[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
+  DeviceGuard guard(h->cfg.device);
+  return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
+                 1.0, nullptr, nullptr, &po);
 }
 
 int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, void* obs_out, void* ref_out, void* reward_out,

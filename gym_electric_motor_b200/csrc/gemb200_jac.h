@@ -1,5 +1,6 @@
-// gemb200_jac.h — the rollout-Jacobian launch (gemb200_rollout_jacobians) as the host unit sees it.  The kernels live in
-// gemb200_tangent.cuh and are instantiated per (motor family, real) in gemb200_jac_tu.cu.
+// gemb200_jac.h — the rollout-Jacobian launch (gemb200_rollout_jacobians), the return-gradient launch and the parameter-sensitivity launch
+// as the host unit sees them.  The kernels live in gemb200_tangent.cuh and are instantiated per (motor family, real) in gemb200_jac_tu.cu,
+// gemb200_grad_tu.cu and gemb200_psens_tu.cu.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -33,5 +34,19 @@ struct GradOut {
 };
 
 template <int FAM, typename real> cudaError_t launch_grad_f(int nref, const StepParams<real>& p, const GradOut& go, cudaStream_t st);
+
+// Where the parameter sensitivities of gemb200_rollout_param_sens go, and with respect to what.  sio: S = d x / d theta [N][n_x][n_p], read
+// at the start of the launch and overwritten with its value after the last step; sout: S after every step [K][N][n_x][n_p], or NULL; slot[c]:
+// the parameter row slot of column c; raw: the configuration's parameter row (the envs' parameters when the handle has no per-env blocks).
+constexpr int kMaxSensParams = 12;
+struct PsOut {
+  void* sio;
+  void* sout;
+  int np;
+  int32_t slot[kMaxSensParams];
+  double raw[kMaxDraw];
+};
+
+template <int FAM, typename real> cudaError_t launch_psens_f(bool finite, int nref, const StepParams<real>& p, const PsOut& po, cudaStream_t st);
 
 }  // namespace gemb200

@@ -88,41 +88,67 @@ template <int FAM, typename real> struct TanIM {  // SCIM, and DFIM with its rot
 template <typename real> struct Tan<kSCIM, real> : TanIM<kSCIM, real> {};
 template <typename real> struct Tan<kDFIM, real> : TanIM<kDFIM, real> {};
 
-// rk4_step with its tangent: x, dx advance together; dws accumulates the tangent of the omega sum with the weights 1-2-2-1
+// Parameter sensitivities: adds to d the derivative of Model<FAM>::rhs along a coefficient tangent tk at fixed (x, u), u = the solver-frame
+// voltages.  The electrical rows and the voltage terms are linear in the coefficients (the DFIM's rotor voltages enter without one); the
+// mechanical row inv_j (T(tq, x) - T_L(a, b, c, omega_lin)) takes the product rule, on the static-friction branch the primal takes.
 template <int FAM, typename real>
+__device__ __forceinline__ void coef_rhs_t(const Coef<real>& kc, const Coef<real>& tk, const real* x, const real* u, int mech, real* d) {
+  constexpr int NX = Fam<FAM>::NX;
+  real ub[4], e[NX];
+  Model<FAM, real>::ubias(tk, u, ub);
+  if constexpr (FAM == kDFIM) { ub[2] = real(0); ub[3] = real(0); }
+  Model<FAM, real>::rhs(tk, real(0), x, ub, 0, real(0), e);
+#pragma unroll
+  for (int j = 1; j < NX; ++j) d[j] += e[j];
+  if (mech == 1) {
+    const real w = x[0], sign = sgn(w);
+    const bool slide = Num<real>::abs(w) > kc.omega_lim;
+    const real tl = fm(sign * kc.load_c * w, w, fm(kc.load_b, w, slide ? sign * kc.load_a : kc.omega_lin * w));
+    const real dtl = fm(sign * tk.load_c * w, w, fm(tk.load_b, w, slide ? sign * tk.load_a : tk.omega_lin * w));
+    d[0] += tk.inv_j * (Model<FAM, real>::torque(kc, x) - tl) + kc.inv_j * (Model<FAM, real>::torque(tk, x) - dtl);
+  }
+}
+
+// rk4_step with its tangent: x, dx advance together; dws accumulates the tangent of the omega sum with the weights 1-2-2-1.
+// PS (parameter sensitivities): the tangent also carries the coefficient tangent tk at the solver-frame voltages us
+template <int FAM, typename real, bool PS = false>
 __device__ __forceinline__ void rk4_step_t(const StepParams<real>& p, const Coef<real>& kc, real* x, real* dx, const real* ub, const real* dub, real h, int mech,
-                                           real& dws, const real* gt) {
+                                           real& dws, const real* gt, const Coef<real>* tk = nullptr, const real* us = nullptr) {
   constexpr int NX = Fam<FAM>::NX;
   const real hh = real(0.5) * h, h6 = h * real(1.0 / 6.0);
   const real g0 = mech == 2 ? gt[0] : real(0), g1 = mech == 2 ? gt[1] : real(0), g2 = mech == 2 ? gt[2] : real(0);
   real k[NX], dk[NX], acc[NX], dacc[NX], xt[NX], dxt[NX];
   Model<FAM, real>::rhs(kc, p.ext_inv_tau, x, ub, mech, g0, k);
   Tan<FAM, real>::rhs(kc, p.ext_inv_tau, x, dx, dub, mech, dk);
+  if constexpr (PS) coef_rhs_t<FAM, real>(kc, *tk, x, us, mech, dk);
   if (mech) dws += dx[0];
   acc[0] = real(0); dacc[0] = real(0); xt[0] = x[0]; dxt[0] = dx[0];
 #pragma unroll
   for (int j = 0; j < NX; ++j) if (j > 0 || mech) { acc[j] = k[j]; dacc[j] = dk[j]; xt[j] = fm(hh, k[j], x[j]); dxt[j] = fm(hh, dk[j], dx[j]); }
   Model<FAM, real>::rhs(kc, p.ext_inv_tau, xt, ub, mech, g1, k);
   Tan<FAM, real>::rhs(kc, p.ext_inv_tau, xt, dxt, dub, mech, dk);
+  if constexpr (PS) coef_rhs_t<FAM, real>(kc, *tk, xt, us, mech, dk);
   if (mech) dws += real(2) * dxt[0];
 #pragma unroll
   for (int j = 0; j < NX; ++j) if (j > 0 || mech) { acc[j] = fm(real(2), k[j], acc[j]); dacc[j] = fm(real(2), dk[j], dacc[j]); xt[j] = fm(hh, k[j], x[j]); dxt[j] = fm(hh, dk[j], dx[j]); }
   Model<FAM, real>::rhs(kc, p.ext_inv_tau, xt, ub, mech, g1, k);
   Tan<FAM, real>::rhs(kc, p.ext_inv_tau, xt, dxt, dub, mech, dk);
+  if constexpr (PS) coef_rhs_t<FAM, real>(kc, *tk, xt, us, mech, dk);
   if (mech) dws += real(2) * dxt[0];
 #pragma unroll
   for (int j = 0; j < NX; ++j) if (j > 0 || mech) { acc[j] = fm(real(2), k[j], acc[j]); dacc[j] = fm(real(2), dk[j], dacc[j]); xt[j] = fm(h, k[j], x[j]); dxt[j] = fm(h, dk[j], dx[j]); }
   Model<FAM, real>::rhs(kc, p.ext_inv_tau, xt, ub, mech, g2, k);
   Tan<FAM, real>::rhs(kc, p.ext_inv_tau, xt, dxt, dub, mech, dk);
+  if constexpr (PS) coef_rhs_t<FAM, real>(kc, *tk, xt, us, mech, dk);
   if (mech) dws += dxt[0];
 #pragma unroll
   for (int j = 0; j < NX; ++j) if (j > 0 || mech) { x[j] = fm(h6, acc[j] + k[j], x[j]); dx[j] = fm(h6, dacc[j] + dk[j], dx[j]); }
 }
 
 // integrate with its tangent over one segment; returns the tangent of the omega sum (the angle advances by kang * wsum)
-template <int FAM, typename real>
+template <int FAM, typename real, bool PS = false>
 __device__ __forceinline__ real integrate_t(const StepParams<real>& p, const Coef<real>& kc, real* x, real* dx, const real* ub, const real* dub, real h_seg, int mech,
-                                            const real* gt) {
+                                            const real* gt, const Coef<real>* tk = nullptr, const real* us = nullptr) {
   constexpr int NX = Fam<FAM>::NX;
   real dws = mech ? real(0) : dx[0];  // constant speed: the sum is omega itself
   const int ns = p.nsteps;
@@ -133,6 +159,7 @@ __device__ __forceinline__ real integrate_t(const StepParams<real>& p, const Coe
       real d[NX], dd[NX];
       Model<FAM, real>::rhs(kc, p.ext_inv_tau, x, ub, mech, mech == 2 ? gt[ns > 1 ? 2 * ns + 2 * (s + 1) : 0] : real(0), d);  // (the nsteps quirk)
       Tan<FAM, real>::rhs(kc, p.ext_inv_tau, x, dx, dub, mech, dd);
+      if constexpr (PS) coef_rhs_t<FAM, real>(kc, *tk, x, us, mech, dd);
       if (mech) dws += dx[0];
 #pragma unroll
       for (int j = 0; j < NX; ++j) if (j > 0 || mech) { x[j] = fm(d[j], h, x[j]); dx[j] = fm(dd[j], h, dx[j]); }
@@ -140,7 +167,7 @@ __device__ __forceinline__ real integrate_t(const StepParams<real>& p, const Coe
     return dws;
   }
 #pragma unroll 1
-  for (int s = 0; s < ns; ++s) rk4_step_t<FAM, real>(p, kc, x, dx, ub, dub, h, mech, dws, gt + 2 * s);
+  for (int s = 0; s < ns; ++s) rk4_step_t<FAM, real, PS>(p, kc, x, dx, ub, dub, h, mech, dws, gt + 2 * s, tk, us);
   return dws;
 }
 
@@ -410,14 +437,34 @@ __device__ __forceinline__ real reward_t(const StepParams<real>& p, const Coef<r
   return dr;
 }
 
+// Parameter sensitivities: the words of the coefficient block (Coef, kCoefWords) that family FAM reads — load_coef's c and tq words and the
+// six load / inertia words — kept per parameter column in the staging row; word w of that compact list is word ps_word<FAM>(w) of Coef
+template <int FAM> __host__ __device__ constexpr int ps_ncw() { return FAM == kDC1 ? 4 : (FAM == kDC2 ? 5 : (FAM == kSYNC ? 7 : (FAM == kEESM ? 14 : 10))); }
+template <int FAM> __host__ __device__ constexpr int ps_ntq() { return (FAM == kDC2 || FAM == kSCIM || FAM == kDFIM) ? 1 : 2; }
+template <int FAM> __host__ __device__ constexpr int ps_words() { return ps_ncw<FAM>() + ps_ntq<FAM>() + 6; }
+template <int FAM> __host__ __device__ constexpr int ps_word(int w) { return w < ps_ncw<FAM>() ? w : (w < ps_ncw<FAM>() + ps_ntq<FAM>() ? 20 + w - ps_ncw<FAM>() : 24 + w - ps_ncw<FAM>() - ps_ntq<FAM>()); }
+template <int FAM, typename real>
+__device__ __forceinline__ void ps_coef(const real* t, Coef<real>& tk) {
+#pragma unroll
+  for (int w = 0; w < ps_ncw<FAM>(); ++w) tk.c[w] = t[w];
+#pragma unroll
+  for (int w = 0; w < ps_ntq<FAM>(); ++w) tk.tq[w] = t[ps_ncw<FAM>() + w];
+  const real* m = t + ps_ncw<FAM>() + ps_ntq<FAM>();
+  tk.load_a = m[0]; tk.load_b = m[1]; tk.load_c = m[2]; tk.inv_j = m[3]; tk.omega_lim = m[4]; tk.omega_lin = m[5];
+}
+
 // The tangent pass of one step of env i: writes column c of [jac_x | jac_u] for every seed c
 // into this thread's staging row, jac_x row-major at jrow[r * NX1 + c], jac_u row-major at jrow[NX1 * NX1 + r * nu + c - NX1].
 // RW (continuous converters, return_grad_kernel): also d(g^k r_k) / d(x, a) at jrow[NX1 * (NX1 + nu) + c], from the reward-row input rw;
 // the supply voltage and the speed-profile cursor then come from rw too (the pass runs after env_step, on copies of the pre-step state).
-template <int FAM, bool FINITE, typename real, bool RW = false>
+// PS (param_sens_kernel): nu = n_p parameter columns instead; jrow holds S = d x / d theta row-major [NX1][n_p], and column c's pass is seeded
+// with S[:, c], no action tangent and the coefficient tangent tks[c * ps_words<FAM>() ..] (ps_coef), and overwrites S[:, c] with
+// S_{k+1}[:, c] = J_x S_k[:, c] + d x_{k+1} / d theta_c.
+template <int FAM, bool FINITE, typename real, bool RW = false, bool PS = false>
 __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Coef<real>& kc, const real (&x0)[Fam<FAM>::NX], const Ang<real>& ang, const Act<real>& act,
-                                             const unsigned i, const int nu, real* jrow, const RwTan<real>* rw = nullptr) {
+                                             const unsigned i, const int nu, real* jrow, const RwTan<real>* rw = nullptr, const real* tks = nullptr) {
   static_assert(!(RW && FINITE), "return gradients: continuous converters only");
+  static_assert(!(RW && PS), "return gradients and parameter sensitivities are separate kernels");
   using F = Fam<FAM>;
   constexpr int NX = F::NX, NX1 = NX + (F::EPS ? 1 : 0);
   const int mech = p.load_kind == GEMB200_LOAD_CONST_SPEED ? 0 : (p.load_kind == GEMB200_LOAD_EXT_SPEED ? 2 : 1);
@@ -530,19 +577,28 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
     if (r2p > real(0)) { const real ir = Num<real>::rsqrt(r2p); csf = x0[3] * ir; snf = x0[4] * ir; }
   }
   // ---------------- one tangent pass per seed column ----------------
-  const int ncol = NX1 + nu;
+  const int ncol = PS ? nu : NX1 + nu;
 #pragma unroll 1
   for (int c = 0; c < ncol; ++c) {
     real x[NX], dx[NX];
+    real de;  // tangent of the angle (rad), seeded in its own column
+    Coef<real> tk{};  // PS: the column's coefficient tangent
+    if constexpr (PS) {
 #pragma unroll
-    for (int j = 0; j < NX; ++j) { x[j] = x0[j]; dx[j] = c == j ? real(1) : real(0); }
-    real de = (F::EPS && c == NX) ? real(1) : real(0);  // tangent of the angle (rad), seeded in its own column
+      for (int j = 0; j < NX; ++j) { x[j] = x0[j]; dx[j] = jrow[j * nu + c]; }
+      de = F::EPS ? jrow[NX * nu + c] : real(0);
+      ps_coef<FAM, real>(tks + c * ps_words<FAM>(), tk);
+    } else {
+#pragma unroll
+      for (int j = 0; j < NX; ++j) { x[j] = x0[j]; dx[j] = c == j ? real(1) : real(0); }
+      de = (F::EPS && c == NX) ? real(1) : real(0);
+    }
     const real de0 = de;
     real dphi = real(0);  // RW: the field angle's tangent
     if constexpr (RW && (FAM == kSCIM || FAM == kDFIM)) dphi = r2p > real(0) ? (x0[3] * dx[4] - x0[4] * dx[3]) / r2p : real(0);
     real da[GEMB200_MAX_ACT];
 #pragma unroll
-    for (int j = 0; j < GEMB200_MAX_ACT; ++j) da[j] = c - NX1 == j ? real(1) : real(0);
+    for (int j = 0; j < GEMB200_MAX_ACT; ++j) da[j] = (!PS && c - NX1 == j) ? real(1) : real(0);
     if constexpr (!FINITE && (FAM == kSYNC || FAM == kEESM || FAM == kSCIM)) {
       if (dq) {  // a_abc = T32 rot(theta) a_dq: theta = eps + angle_advance tau p omega, or (SCIM) the field angle of the flux
         real dth;
@@ -593,10 +649,14 @@ __device__ __forceinline__ void step_tangent(const StepParams<real>& p, const Co
       }
       real dub[4];
       Model<FAM, real>::ubias(kc, dus, dub);
-      dws = integrate_t<FAM, real>(p, kc, x, dx, ubg[seg], dub, hsg[seg], mech, gt);
+      dws = integrate_t<FAM, real, PS>(p, kc, x, dx, ubg[seg], dub, hsg[seg], mech, gt, &tk, usg[seg]);
       if constexpr (F::EPS) de = fm(kag[seg], dws, de);  // the wrap to (-pi, pi] has derivative 1
     }
-    if (c < NX1) {
+    if constexpr (PS) {
+#pragma unroll
+      for (int r = 0; r < NX; ++r) jrow[r * nu + c] = dx[r];
+      if constexpr (F::EPS) jrow[NX * nu + c] = de;
+    } else if (c < NX1) {
 #pragma unroll
       for (int r = 0; r < NX; ++r) jrow[r * NX1 + c] = dx[r];
       if constexpr (F::EPS) jrow[NX * NX1 + c] = de;
@@ -924,6 +984,132 @@ return_grad_kernel(const __grid_constant__ StepParams<real> p, const __grid_cons
     if constexpr (F::EPS) ang.store(p.eps, i);
     p.ret_out[i] = acc.g;
     if (p.ret_end) p.ret_end[i] = acc.end;
+  }
+}
+
+// The K-step loop of param_sens_kernel: jac_loop's steps with the parameter column passes instead of the seed columns.  The thread's
+// staging row holds S [NX1][n_p] (loaded from sens_io, stored back after the last step) and behind it the coefficient tangents of the n_p
+// columns (ps_words<FAM>() words each).  Step k: the column passes advance S to S_{k+1} on the pre-step state, env_step advances the primal,
+// S_{k+1} goes to sens_out[k], and an env that env_step has just reset (autoreset same_step) restarts from S = 0: its reset state does not
+// depend on theta.
+template <int FAM, bool FINITE, typename real, int NREF, bool ENVP>
+__device__ __forceinline__ void psens_loop(const StepParams<real>& p, const PsOut& po, CoefArg<real, ENVP> kc, const unsigned i, const bool active, real (&x)[Fam<FAM>::NX],
+                                           Ang<real>& ang, real (&rv)[NREF > 0 ? NREF : 1], real (&rs)[NREF > 0 ? NREF : 1], uint32_t (&rend)[NREF > 0 ? NREF : 1],
+                                           bool& cold_dirty, real* rows, real* row, real* jrows, real* jrow, const int jstride, const int lane, const int stride) {
+  constexpr int NX1 = Fam<FAM>::NX + (Fam<FAM>::EPS ? 1 : 0);
+  const int K = p.roll_steps;
+  const int np = po.np, ws = NX1 * np;
+  const size_t n = (size_t)(unsigned)p.n;
+  Out<real> out = make_out<NREF, false, real>(p, i, lane, p.n_obs);
+  ClockArg<ENVP> ck = clock_of(p);
+  if constexpr (ENVP) ck = id_clock(p, clock_of(p), active ? i : (unsigned)p.env_begin);
+  const char* act = action_cursor<FAM, FINITE, real, false>(p, p.action, i);
+  WalkCache wc{};
+  Act<real> a_next{};
+  if (active) a_next = load_action<FAM, FINITE, real, false>(p, act);
+  constexpr bool kFeed = NREF > 0;
+  const bool feed = kFeed && p.ref_feed != nullptr;
+  const real* fc = nullptr;
+  real f_next[NREF > 0 ? NREF : 1];
+  if constexpr (kFeed) {
+    if (feed) { fc = feed_cursor<NREF, false, real>(p, i); if (active) load_feed<NREF, false, real>(p, fc, f_next); }
+  }
+  const size_t warp_env0 = i - lane;
+  real* sio = static_cast<real*>(po.sio) + warp_env0 * (size_t)ws;
+  real* so = po.sout ? static_cast<real*>(po.sout) + warp_env0 * (size_t)ws : nullptr;
+  const real* tks = jrow + ws;
+  warp_load_jac(jrows, sio, jstride, ws, out.valid, lane);
+  __syncwarp();
+#pragma unroll 1
+  for (int k = 0; k < K; ++k) {
+    const Act<real> a_cur = a_next;
+    act += p.roll_act_inc;
+    if (active && k + 1 < K) a_next = load_action<FAM, FINITE, real, false>(p, act);
+    if constexpr (kFeed) {
+      if (feed) {
+#pragma unroll
+        for (int r = 0; r < NREF; ++r) rv[r] = f_next[r];
+        fc += n * NREF;
+        if (active && k + 1 < K) load_feed<NREF, false, real>(p, fc, f_next);
+      }
+    }
+    if (active) step_tangent<FAM, FINITE, real, false, true>(p, kc, x, ang, a_cur, i, np, jrow, nullptr, tks);
+    const StepOut<real> sto = env_step<FAM, FINITE, real, NREF, false, false, false, false, ENVP>(p, kc, ck, out, true, a_cur, i, active, x, ang, rv, rs, rend,
+                                                                                                cold_dirty, wc, rows, row, lane, stride);
+    __syncwarp();
+    if (so) {
+      warp_store_jac(so, jrows, jstride, ws, out.valid, lane);
+      so += n * (size_t)ws;
+      __syncwarp();
+    }
+    if (active && sto.term && p.autoreset == GEMB200_AUTORESET_SAME_STEP)
+      for (int w = 0; w < ws; ++w) jrow[w] = real(0);
+    __syncwarp();  // the observation rows are reused by the next step
+    out.obs = byte_add(out.obs, p.roll_obs_inc); out.ref = byte_add(out.ref, p.roll_ref_inc);
+    out.rew = byte_add(out.rew, p.roll_rew_inc); out.term = byte_add(out.term, p.roll_term_inc);
+    ck.kstep += 1u;
+    ck.gstep_lo += 1u;
+    if (ck.gstep_lo == 0u) ck.gstep_hi += 1u;
+  }
+  warp_store_jac(sio, jrows, jstride, ws, out.valid, lane);
+}
+
+// The parameter-sensitivity kernel: jacobian_kernel's shape with psens_loop.  Before the loop every env derives the coefficient tangents
+// of its n_p parameters once, in double precision (coef_tangent, gemb200_model.h), from its own parameter row (ENVP: praw) or the
+// configuration's (po.raw), into its staging row.  Dynamic shared memory: the observation rows of the block, then per env its row of S and
+// coefficient tangents (jstride words).
+template <int FAM, bool FINITE, typename real, int NREF, bool ENVP>
+__global__ void __launch_bounds__(GEMB200_BLOCK, (sizeof(real) == 4 ? GEMB200_MINBLOCKS_JAC : GEMB200_MINBLOCKS_JAC_F64))
+param_sens_kernel(const __grid_constant__ StepParams<real> p, const __grid_constant__ PsOut po, const int jstride) {
+  using F = Fam<FAM>;
+  constexpr int NX = F::NX, NX1 = NX + (F::EPS ? 1 : 0), NH = hot_words(NX, NREF), NC = cold_words(NX, NREF), NW = ps_words<FAM>();
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  real* smem = reinterpret_cast<real*>(smem_raw);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int stride = p.row_stride;
+  real* rows = smem + warp * (32 * stride);
+  real* row = rows + lane * stride;
+  real* jrows = smem + blockDim.x * stride + warp * (32 * jstride);
+  real* jrow = jrows + lane * jstride;
+  const unsigned i = (unsigned)p.env_begin + blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned n = (unsigned)p.n;
+  const bool active = i < (unsigned)p.env_end;
+  const int mech = p.load_kind != GEMB200_LOAD_CONST_SPEED;
+  real hot[NH > 0 ? NH : 1], cold[NC];
+  Ang<real> ang;
+  real x[NX], rv[NREF > 0 ? NREF : 1], rs[NREF > 0 ? NREF : 1];
+  uint32_t rend[NREF > 0 ? NREF : 1];
+  bool cold_dirty = mech;
+  if (active) {
+    if constexpr (NH > 0) load_words<NH, real>(p.st, i, n, hot);
+    load_words<NC, real>(p.stc, i, n, cold);
+    ang.set(p.init_ang);
+    if constexpr (F::EPS) ang.load(p.eps, i);
+    unpack_records<NX, NREF, real>(hot, cold, x, rv, rs, rend);
+    double prm[kMaxDraw];
+#pragma unroll 1
+    for (int s = 0; s < kMaxDraw; ++s) prm[s] = ENVP ? p.praw[(size_t)s * n + i] : po.raw[s];
+    real* tks = jrow + NX1 * po.np;
+#pragma unroll 1
+    for (int c = 0; c < po.np; ++c) {
+      double t[kCoefWords];
+      coef_tangent(p.motor_kind, prm, po.slot[c], t);
+#pragma unroll
+      for (int w = 0; w < NW; ++w) tks[c * NW + w] = (real)t[ps_word<FAM>(w)];
+    }
+  }
+  if constexpr (ENVP) {
+    Coef<real> kl;
+    load_coef<FAM, real>(p, active ? i : (unsigned)p.env_begin, mech != 0, kl);
+    psens_loop<FAM, FINITE, real, NREF, true>(p, po, kl, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
+  } else {
+    psens_loop<FAM, FINITE, real, NREF, false>(p, po, p.k, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
+  }
+  if (active) {
+    pack_records<NX, NREF, real>(hot, cold, x, rv, rs, rend);
+    if constexpr (NH > 0) store_words<NH, real>(p.st, i, n, hot);
+    if (cold_dirty) store_words<NC, real>(p.stc, i, n, cold);
+    if constexpr (F::EPS) ang.store(p.eps, i);
   }
 }
 

@@ -401,6 +401,72 @@ class VectorSim:
                                                        _ptr(grad_x0), _ptr(obs), _ptr(ref) if self.n_ref else None, self._stream()),
                 "gemb200_rollout_return_grads")
 
+    @staticmethod
+    def _slot_array(slots):
+        slots = [int(v) for v in slots]
+        return (C.c_int32 * max(len(slots), 1))(*slots), len(slots)
+
+    def param_sens_dims(self, slots):
+        """n_x of `rollout_param_sens` for the parameter slots `slots` (GEMB200_MP_* / GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_*): n_ode.
+        NotImplementedError for a refused configuration or slot list (DESIGN.md §7)."""
+        lib = K.load_library()  # a configuration query: no handle, no launch
+        arr, n_p = self._slot_array(slots)
+        nx = C.c_int32()
+        if lib.gemb200_query_param_sens_dims(C.byref(self.cfg), n_p, arr, C.byref(nx)):
+            raise NotImplementedError(lib.gemb200_last_error().decode())
+        return nx.value
+
+    def coef_tangents(self, slots, motor_param=None, load_param=None):
+        """d (coefficient block) / d theta for the slots at a parameter row (the configuration's when None): float64 [n_p, 30] in the word
+        order of the per-env coefficient block (gemb200_coef_tangents; no GPU)."""
+        lib = K.load_library()
+        arr, n_p = self._slot_array(slots)
+        out = np.zeros((n_p, 30), dtype=np.float64)
+        mp = None if motor_param is None else np.ascontiguousarray(motor_param, dtype=np.float64)
+        lp = None if load_param is None else np.ascontiguousarray(load_param, dtype=np.float64)
+        K.check(lib.gemb200_coef_tangents(C.byref(self.cfg), None if mp is None else mp.ctypes.data, None if lp is None else lp.ctypes.data, n_p, arr,
+                                          out.ctypes.data), "gemb200_coef_tangents")
+        return out
+
+    def _as_sens(self, sens, nx, n_p):
+        shape = (self.n, nx, n_p)
+        if (not isinstance(sens, torch.Tensor) or sens.dtype != self.dtype or sens.device != self.device or tuple(sens.shape) != shape
+                or not sens.is_contiguous()):
+            got = f"{tuple(sens.shape)} {sens.dtype} on {sens.device}" if isinstance(sens, torch.Tensor) else type(sens).__name__
+            raise ValueError(f"sens0 must be a contiguous [{self.n}, {nx}, {n_p}] {self.dtype} tensor on {self.device}, got {got}")
+        return sens
+
+    def rollout_param_sens(self, actions, slots, references=None, sens0=None, record=True):
+        """K open-loop steps in ONE launch that also carry the parameter sensitivities S = d x / d theta (gemb200_rollout_param_sens).
+        Returns ((sens, sens_last), (obs, ref, rew, term)): sens [K, N, n_x, n_p] = d x_{k+1} / d theta after every step (None when
+        record=False), sens_last [N, n_x, n_p] = the carried S after the last step (0 for an env reset in it), in the handle's dtype; the
+        outputs of every step exactly as `rollout(actions, record_every=1, references=references)` returns them.  sens0 [N, n_x, n_p]: S at
+        the start (None: zeros); it is not modified.  Refused configurations or slots: NotImplementedError (DESIGN.md §7); bad actions, feed
+        or sens0: ValueError before any launch."""
+        nx = self.param_sens_dims(slots)
+        n_p = len(slots)
+        a = self._as_actions(actions)
+        k = int(a.shape[0])
+        r = None if references is None else self._as_feed(references, k)
+        sio = (torch.zeros((self.n, nx, n_p), dtype=self.dtype, device=self.device) if sens0 is None
+               else self._as_sens(sens0, nx, n_p).clone())
+        so = torch.empty((k, self.n, nx, n_p), dtype=self.dtype, device=self.device) if record else None
+        obs = torch.empty((k,) + self._shape(self.n_state), dtype=self.dtype, device=self.device)
+        ref = torch.empty((k,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device)
+        rew = torch.empty((k, self.n), dtype=self.dtype, device=self.device)
+        term = torch.empty((k, self.n), dtype=torch.uint8, device=self.device)
+        self.rollout_param_sens_into(a, k, slots, sio, so, obs, ref, rew, term, r)
+        return (so, sio), (obs, ref, rew, term)
+
+    def rollout_param_sens_into(self, actions, n_steps, slots, sens_io, sens_out=None, obs=None, ref=None, rew=None, term=None, references=None):
+        """Raw variant of `rollout_param_sens` for benchmarking: caller-owned outputs (all but `sens_io` may be None; sens_io is read as S_0
+        and overwritten with S_K), no allocation, no conversion.  The reference feed is checked like there."""
+        r = None if references is None else self._as_feed(references, n_steps)
+        arr, n_p = self._slot_array(slots)
+        K.check(self._lib.gemb200_rollout_param_sens(self._h, _ptr(actions), _ptr(r), int(n_steps), n_p, arr, _ptr(sens_io), _ptr(sens_out), _ptr(obs),
+                                                     _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term), self._stream()),
+                "gemb200_rollout_param_sens")
+
     # ------------------------------------------------------------------ host-buffer API (numpy)
     def step_host(self, action, out=None):
         """Same step through HOST buffers (the C-ABI does H2D, launch, D2H, sync).  `out` = tuple of numpy arrays to

@@ -369,6 +369,29 @@ int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const v
                                  void* workspace, uint64_t workspace_bytes, void* return_out, int32_t* end_step_out, void* grad_a_out, void* grad_x0_out,
                                  void* obs_out, void* ref_out, void* stream);
 
+/* Parameter sensitivities along a fused rollout: d x_k / d theta of the physical parameters theta, forward mode.  slots[0 .. n_p - 1]: the
+ * parameters, in the slot numbers of a parameter row (GEMB200_MP_* for the motor, GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_* for the load).
+ * Accepted: every motor slot but GEMB200_MP_P (the angle increments are per handle) and GEMB200_MP_K (the EESM's coefficients are invariant
+ * in it), and the load slots A, B, C, J_LOAD; 1 <= n_p <= 12, no slot twice.  A slot that does not enter the configuration's model has
+ * sensitivity 0.  Limits, the normalisation and the FluxObserver constants are held fixed.
+ * gemb200_query_param_sens_dims (needs no GPU): n_x = n_ode as for the Jacobians; GEMB200_E_INVALID for everything
+ * gemb200_query_jacobian_dims refuses and for a refused slot list (DESIGN.md §7).
+ * gemb200_coef_tangents (needs no GPU): out[a][30] = d (coefficient block) / d theta_a at the parameter row (motor_param[16], load_param[8];
+ * NULL: the configuration's), in the word order of the per-env coefficient block: c[20], tq[4], load a, b, c, inv_j, omega_lim, omega_lin
+ * — the derivation the launch runs on the device.
+ * gemb200_rollout_param_sens: n_steps = K open-loop steps in ONE launch; each env is differentiated with respect to its own parameters (its
+ * per-env block, or the configuration's).  sens_io [N][n_x][n_p]: S_0 on entry (zeros: the trajectory from the current state), S_K on
+ * return, so that launches chain.  sens_out [K][N][n_x][n_p] (or NULL): S_{k+1} = d x_{k+1} / d theta after every step k.  x as
+ * gemb200_get_ode_state (the angle last, in radians).  Non-smooth points as for the Jacobians.  A terminating step reports the sensitivity
+ * of the physical step it took; under autoreset same_step the carried S of a reset env then restarts from 0.  obs_out / ref_out / reward_out
+ * / terminated_out, the final state, clock and RNG position are exactly those of gemb200_rollout_record_ref(record_every = 1).  Refused
+ * while parameter draws at resets are on.  All buffers are device memory in the handle's dtype; the call allocates nothing.
+ * Stream-ordered, capturable in a CUDA graph under the device clock. */
+int gemb200_query_param_sens_dims(const gemb200_config* cfg, int32_t n_p, const int32_t* slots, int32_t* n_x);
+int gemb200_coef_tangents(const gemb200_config* cfg, const double* motor_param, const double* load_param, int32_t n_p, const int32_t* slots, double* out);
+int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t n_p, const int32_t* slots,
+                               void* sens_io, void* sens_out, void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream);
+
 /* OdeSolver.y / set_initial_value (physical_systems/solvers.py:4-76): ODE state as double [N][n_ode]
  * (AoS, device), angle unwrapped to (-pi, pi].  Used for checkpointing and oracle injection. */
 int gemb200_get_ode_state(gemb200_handle* h, double* ode_out, void* stream);
