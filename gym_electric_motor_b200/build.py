@@ -3,9 +3,9 @@
     python -m gym_electric_motor_b200.build [--force] [--verbose]
 
 The step kernel's 200 instantiations are spread over twelve translation units (motor family x real, csrc/gemb200_step_tu.cu)
-that compile in parallel, the rollout-Jacobian kernels over twelve more (csrc/gemb200_jac_tu.cu), the return-gradient kernels over another twelve
-(csrc/gemb200_grad_tu.cu) and the parameter-sensitivity kernels over twelve more (csrc/gemb200_psens_tu.cu); objects go to build/ (git-ignored),
-only the linked .so stays in the package.
+that compile in parallel.  The tangent-rollout kernels (csrc/gemb200_tangent.cuh) come from one source, csrc/gemb200_tangent_tu.cu,
+compiled once per kind x family x real (kind = the output struct: JacOut rollout Jacobians, GradOut return gradients, PsOut parameter
+sensitivities), 36 more units; objects go to build/ (git-ignored), only the linked .so stays in the package.
 """
 import hashlib
 import os
@@ -18,8 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 HEADERS = [os.path.join(CSRC, "gemb200_kernels.cuh"), os.path.join(CSRC, "gemb200_params.h"), os.path.join(CSRC, "gemb200_launch.cuh"),
            os.path.join(CSRC, "gemb200_model.h"), os.path.join(CSRC, "gemb200_jac.h"), os.path.join(CSRC, "gemb200_tangent.cuh"),
            os.path.join(HERE, "..", "include", "gemb200.h")]
-SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu"), os.path.join(CSRC, "gemb200_jac_tu.cu"),
-           os.path.join(CSRC, "gemb200_grad_tu.cu"), os.path.join(CSRC, "gemb200_psens_tu.cu")]
+SOURCES = [os.path.join(CSRC, "gemb200.cu"), os.path.join(CSRC, "gemb200_step_tu.cu"), os.path.join(CSRC, "gemb200_tangent_tu.cu")]
 OUT = os.path.join(HERE, "libgemb200.so")
 OBJ_DIR = os.path.join(HERE, "..", "build", "gemb200")
 # -fmad=false: no implicit contraction of a*b+c — every fused multiply-add of the kernels is written out (fm() in gemb200_kernels.cuh), so
@@ -31,6 +30,7 @@ NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-fmad=false", "-Xcompiler", "-fPIC"]
 LINEINFO = ["-lineinfo"]
 FAMILIES = (0, 1, 2, 3, 4, 5)  # gemb200_params.h: MotorFamily
 REALS = ("float", "double")
+TANGENT_KINDS = (("jac", "JacOut"), ("grad", "GradOut"), ("psens", "PsOut"))  # object prefix, output struct (gemb200_jac.h)
 
 
 def nvcc_path():
@@ -54,16 +54,11 @@ def _units(only=None):
             if only and (fam, real) not in only:
                 continue
             units.append((f"step_f{fam}_{real}", SOURCES[1], [f"-DGEMB200_TU_FAM={fam}", f"-DGEMB200_TU_REAL={real}"] + (LINEINFO if real == "float" else [])))
-    if not only:  # the rollout-Jacobian kernels (gemb200_jac_tu.cu): one unit per family x real, like the step kernels
-        for fam in FAMILIES:
-            for real in REALS:
-                units.append((f"jac_f{fam}_{real}", SOURCES[2], [f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
-        for fam in FAMILIES:  # the return-gradient kernels (gemb200_grad_tu.cu), likewise
-            for real in REALS:
-                units.append((f"grad_f{fam}_{real}", SOURCES[3], [f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
-        for fam in FAMILIES:  # the parameter-sensitivity kernels (gemb200_psens_tu.cu), likewise
-            for real in REALS:
-                units.append((f"psens_f{fam}_{real}", SOURCES[4], [f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
+    if not only:  # the tangent-rollout kernels: one unit per kind x family x real, like the step kernels
+        for prefix, out in TANGENT_KINDS:
+            for fam in FAMILIES:
+                for real in REALS:
+                    units.append((f"{prefix}_f{fam}_{real}", SOURCES[2], [f"-DGEMB200_TAN_OUT={out}", f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
     return units
 
 

@@ -9,6 +9,7 @@
 #include <new>
 #include <limits>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "gemb200_jac.h"
@@ -620,91 +621,24 @@ static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
 }
 
 // ----------------------------------------------------------------------------------------------------------------
-// kernel dispatch (the instantiations live in gemb200_step_tu.cu, one TU per family x real)
+// kernel dispatch (the instantiations live in gemb200_step_tu.cu and gemb200_tangent_tu.cu, one TU per family x real and kind)
 // ----------------------------------------------------------------------------------------------------------------
-// GEMB200_ONLY_FAM=<family>: experiment builds (tools/build_variants.py --only) that carry the fp32 kernels of ONE motor family; every
-// other configuration fails with cudaErrorInvalidValue instead of leaving unresolved symbols.  Never defined in the product build.
-template <typename real>
-static cudaError_t launch_step(int fam, bool finite, int nref, const StepParams<real>& p, cudaStream_t st) {
+// launch(std::integral_constant<int, FAM>{}) for motor family fam.  GEMB200_ONLY_FAM=<family>: experiment builds (tools/build_variants.py
+// --only) that carry the fp32 step and reset kernels of ONE motor family and no tangent kernels (TANGENT: a tangent-rollout launch); every
+// other launch fails with cudaErrorInvalidValue instead of leaving unresolved symbols.  Never defined in the product build.
+template <bool TANGENT, typename real, typename L>
+static cudaError_t for_family(int fam, L&& launch) {
 #ifdef GEMB200_ONLY_FAM
-  if constexpr (std::is_same<real, float>::value) { if (fam == GEMB200_ONLY_FAM) return launch_step_f<GEMB200_ONLY_FAM, real>(finite, nref, p, st); }
+  if constexpr (!TANGENT && std::is_same<real, float>::value) { if (fam == GEMB200_ONLY_FAM) return launch(std::integral_constant<int, GEMB200_ONLY_FAM>{}); }
   return cudaErrorInvalidValue;
 #else
   switch (fam) {
-    case kDC1: return launch_step_f<kDC1, real>(finite, nref, p, st);
-    case kDC2: return launch_step_f<kDC2, real>(finite, nref, p, st);
-    case kSYNC: return launch_step_f<kSYNC, real>(finite, nref, p, st);
-    case kEESM: return launch_step_f<kEESM, real>(finite, nref, p, st);
-    case kSCIM: return launch_step_f<kSCIM, real>(finite, nref, p, st);
-    case kDFIM: return launch_step_f<kDFIM, real>(finite, nref, p, st);
-  }
-  return cudaErrorInvalidValue;
-#endif
-}
-template <typename real>
-static cudaError_t launch_reset(int fam, int nref, const StepParams<real>& p, cudaStream_t st) {
-#ifdef GEMB200_ONLY_FAM
-  if constexpr (std::is_same<real, float>::value) { if (fam == GEMB200_ONLY_FAM) return launch_reset_f<GEMB200_ONLY_FAM, real>(nref, p, st); }
-  return cudaErrorInvalidValue;
-#else
-  switch (fam) {
-    case kDC1: return launch_reset_f<kDC1, real>(nref, p, st);
-    case kDC2: return launch_reset_f<kDC2, real>(nref, p, st);
-    case kSYNC: return launch_reset_f<kSYNC, real>(nref, p, st);
-    case kEESM: return launch_reset_f<kEESM, real>(nref, p, st);
-    case kSCIM: return launch_reset_f<kSCIM, real>(nref, p, st);
-    case kDFIM: return launch_reset_f<kDFIM, real>(nref, p, st);
-  }
-  return cudaErrorInvalidValue;
-#endif
-}
-
-template <typename real>
-static cudaError_t launch_jac(int fam, bool finite, int nref, const StepParams<real>& p, const JacOut& jo, cudaStream_t st) {
-#ifdef GEMB200_ONLY_FAM
-  return cudaErrorInvalidValue;
-#else
-  switch (fam) {
-    case kDC1: return launch_jac_f<kDC1, real>(finite, nref, p, jo, st);
-    case kDC2: return launch_jac_f<kDC2, real>(finite, nref, p, jo, st);
-    case kSYNC: return launch_jac_f<kSYNC, real>(finite, nref, p, jo, st);
-    case kEESM: return launch_jac_f<kEESM, real>(finite, nref, p, jo, st);
-    case kSCIM: return launch_jac_f<kSCIM, real>(finite, nref, p, jo, st);
-    case kDFIM: return launch_jac_f<kDFIM, real>(finite, nref, p, jo, st);
-  }
-  return cudaErrorInvalidValue;
-#endif
-}
-
-template <typename real>
-static cudaError_t launch_grad(int fam, int nref, const StepParams<real>& p, const GradOut& go, cudaStream_t st) {
-#ifdef GEMB200_ONLY_FAM
-  return cudaErrorInvalidValue;
-#else
-  switch (fam) {
-    case kDC1: return launch_grad_f<kDC1, real>(nref, p, go, st);
-    case kDC2: return launch_grad_f<kDC2, real>(nref, p, go, st);
-    case kSYNC: return launch_grad_f<kSYNC, real>(nref, p, go, st);
-    case kEESM: return launch_grad_f<kEESM, real>(nref, p, go, st);
-    case kSCIM: return launch_grad_f<kSCIM, real>(nref, p, go, st);
-    case kDFIM: return launch_grad_f<kDFIM, real>(nref, p, go, st);
-  }
-  return cudaErrorInvalidValue;
-#endif
-}
-
-template <typename real>
-static cudaError_t launch_psens(int fam, bool finite, int nref, const StepParams<real>& p, const PsOut& po, cudaStream_t st) {
-#ifdef GEMB200_ONLY_FAM
-  return cudaErrorInvalidValue;
-#else
-  switch (fam) {
-    case kDC1: return launch_psens_f<kDC1, real>(finite, nref, p, po, st);
-    case kDC2: return launch_psens_f<kDC2, real>(finite, nref, p, po, st);
-    case kSYNC: return launch_psens_f<kSYNC, real>(finite, nref, p, po, st);
-    case kEESM: return launch_psens_f<kEESM, real>(finite, nref, p, po, st);
-    case kSCIM: return launch_psens_f<kSCIM, real>(finite, nref, p, po, st);
-    case kDFIM: return launch_psens_f<kDFIM, real>(finite, nref, p, po, st);
+    case kDC1: return launch(std::integral_constant<int, kDC1>{});
+    case kDC2: return launch(std::integral_constant<int, kDC2>{});
+    case kSYNC: return launch(std::integral_constant<int, kSYNC>{});
+    case kEESM: return launch(std::integral_constant<int, kEESM>{});
+    case kSCIM: return launch(std::integral_constant<int, kSCIM>{});
+    case kDFIM: return launch(std::integral_constant<int, kDFIM>{});
   }
   return cudaErrorInvalidValue;
 #endif
@@ -754,14 +688,13 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
 // the chunks of one pipelined host step share them.  roll > 0: `roll` fused steps (rollout_kernel) whose call ids, step clock and
 // dead-time ring positions are exactly those of `roll` consecutive single-step calls; outputs every `every` steps (0: last only).
 // feed: the reference values of every step (StepParams::ref_feed), or NULL.  ret / ret_end / discount: the discounted returns of a
-// rollout (StepParams::ret_out), or NULL.  jac: the Jacobian outputs of gemb200_rollout_jacobians, or NULL; with them the launch takes the
-// rollout-Jacobian kernel (gemb200_tangent.cuh) instead of the step / rollout kernels.  grad: the outputs of gemb200_rollout_return_grads,
-// or NULL; with them the launch takes the return-gradient kernel (gemb200_tangent.cuh).  ps: the parameter-sensitivity outputs of
-// gemb200_rollout_param_sens, or NULL; with them the launch takes the parameter-sensitivity kernel (gemb200_tangent.cuh).
+// rollout (StepParams::ret_out), or NULL.  tan: the outputs of a tangent rollout (JacOut: gemb200_rollout_jacobians, GradOut:
+// gemb200_rollout_return_grads, PsOut: gemb200_rollout_param_sens), or NULL; with them the launch takes that kind's kernel
+// (gemb200_tangent.cuh) instead of the step / rollout kernels.
+template <typename TanOut = void>
 static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, void* rew, uint8_t* term, cudaStream_t st,
                    int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr,
-                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const JacOut* jac = nullptr, const GradOut* grad = nullptr,
-                   const PsOut* ps = nullptr) {
+                   void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const TanOut* tan = nullptr) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
@@ -780,10 +713,11 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     p.ref_feed = static_cast<const real*>(feed);
     p.ret_out = static_cast<real*>(ret); p.ret_end = ret_end; p.discount = (real)discount;
     set_roll_strides(h, p);
-    if (jac) return launch_jac<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, *jac, st);
-    if (grad) return launch_grad<real>(h->fam, h->n_ref, p, *grad, st);
-    if (ps) return launch_psens<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, *ps, st);
-    return launch_step<real>(h->fam, h->cfg.finite != 0, h->n_ref, p, st);
+    const bool finite = h->cfg.finite != 0;
+    if constexpr (!std::is_void<TanOut>::value) {
+      if (tan) return for_family<true, real>(h->fam, [&](auto f) { return launch_tangent_f<decltype(f)::value, real>(finite, h->n_ref, p, *tan, st); });
+    }
+    return for_family<false, real>(h->fam, [&](auto f) { return launch_step_f<decltype(f)::value, real>(finite, h->n_ref, p, st); });
   });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string(roll > 0 ? "rollout launch: " : "step launch: ") + cudaGetErrorString(e));
   h->launches += 1;
@@ -801,7 +735,7 @@ static int do_reset(gemb200_handle* h, const uint8_t* mask, void* obs, void* ref
     p.clock_dev = dev_clock ? h->d_clock : nullptr;
     p.gstep_lo = (uint32_t)h->gstep; p.gstep_hi = (uint32_t)(h->gstep >> 32);
     p.reset_mask = mask; p.obs = (real*)obs; p.ref_out = (real*)ref; p.kstep = dev_clock ? 0u : (uint32_t)h->n_steps;
-    const cudaError_t le = launch_reset<real>(h->fam, h->n_ref, p, st);
+    const cudaError_t le = for_family<false, real>(h->fam, [&](auto f) { return launch_reset_f<decltype(f)::value, real>(h->n_ref, p, st); });
     p.reset_mask = nullptr;
     return le;
   });
@@ -845,6 +779,17 @@ static int launch_accessor(gemb200_handle* h, void* stream, F&& launch) {
 // ----------------------------------------------------------------------------------------------------------------
 // C-ABI
 // ----------------------------------------------------------------------------------------------------------------
+// The checks the rollout entry points share, behind the handle check and each entry's own checks, in the order they fail: n_steps, then
+// the entry's check that must fail right after it (`after_n_steps`: its message when it fails, else NULL; record_every reads n_steps), then
+// the reference feed
+static int check_rollout(const gemb200_handle* h, int32_t n_steps, const void* references, const char* after_n_steps = nullptr) {
+  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
+  if (after_n_steps) return fail(GEMB200_E_INVALID, after_n_steps);
+  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  return GEMB200_OK;
+}
+static const char* check_discount(double discount) { return discount >= 0.0 && discount <= 1.0 ? nullptr : "discount must be finite and in [0, 1]"; }
+
 extern "C" {
 
 int gemb200_version(void) { return GEMB200_ABI_VERSION; }
@@ -1100,9 +1045,8 @@ int gemb200_rollout_record(gemb200_handle* h, const void* actions, int32_t n_ste
 int gemb200_rollout_record_ref(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t record_every,
                                void* obs_out, void* ref_out, void* reward_out, uint8_t* terminated_out, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
-  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
-  if (record_every < 0 || record_every > n_steps) return fail(GEMB200_E_INVALID, "record_every must be in [0, n_steps]");
-  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  const char* every = record_every < 0 || record_every > n_steps ? "record_every must be in [0, n_steps]" : nullptr;
+  if (int rc = check_rollout(h, n_steps, references, every)) return rc;
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, record_every, references);
 }
@@ -1111,9 +1055,7 @@ int gemb200_rollout_returns(gemb200_handle* h, const void* actions, const void* 
                             void* return_out, int32_t* end_step_out, void* obs_out, void* ref_out, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (!return_out) return fail(GEMB200_E_INVALID, "return_out is NULL");
-  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
-  if (!(discount >= 0.0 && discount <= 1.0)) return fail(GEMB200_E_INVALID, "discount must be finite and in [0, 1]");
-  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  if (int rc = check_rollout(h, n_steps, references, check_discount(discount))) return rc;
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, nullptr, nullptr, (cudaStream_t)stream, 0, -1, true, n_steps, 0, references, return_out,
                  end_step_out, discount);
@@ -1124,8 +1066,7 @@ int gemb200_rollout_jacobians(gemb200_handle* h, const void* actions, const void
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (const char* why = jacobian_refusal(&h->cfg)) return fail(GEMB200_E_INVALID, why);
   if (!jac_x_out) return fail(GEMB200_E_INVALID, "jac_x_out is NULL");
-  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
-  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  if (int rc = check_rollout(h, n_steps, references)) return rc;
   const JacOut jo{jac_x_out, h->cfg.finite ? nullptr : jac_u_out, h->cfg.finite ? 0 : h->n_act};
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
@@ -1143,9 +1084,7 @@ int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const v
   if (!grad_a_out) return fail(GEMB200_E_INVALID, "grad_a_out is NULL");
   if (!grad_x0_out) return fail(GEMB200_E_INVALID, "grad_x0_out is NULL");
   if (!workspace) return fail(GEMB200_E_INVALID, "workspace is NULL");
-  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
-  if (!(discount >= 0.0 && discount <= 1.0)) return fail(GEMB200_E_INVALID, "discount must be finite and in [0, 1]");
-  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  if (int rc = check_rollout(h, n_steps, references, check_discount(discount))) return rc;
   const uint64_t words = (uint64_t)(d.n_ode * (d.n_ode + d.n_act) + d.n_ode + d.n_act);
   const uint64_t need = (uint64_t)n_steps * (uint64_t)h->cfg.n_envs * words * (uint64_t)h->rsz;
   if (workspace_bytes < need) return fail(GEMB200_E_INVALID, "workspace too small: it needs n_steps * n_envs * ws_words * sizeof(real) bytes (gemb200_query_return_grad_dims)");
@@ -1165,7 +1104,7 @@ int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const v
   }
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, nullptr, nullptr, (cudaStream_t)stream, 0, -1, true, n_steps, 0, references, return_out, end_step_out,
-                 discount, nullptr, &go);
+                 discount, &go);
 }
 
 int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const void* references, int32_t n_steps, int32_t n_p, const int32_t* slots,
@@ -1175,8 +1114,7 @@ int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const voi
   if (draws_on(h))
     return fail(GEMB200_E_INVALID, "parameter sensitivities: parameter draws at resets are on, the parameters would change inside the launch (DESIGN.md §7)");
   if (!sens_io) return fail(GEMB200_E_INVALID, "sens_io is NULL");
-  if (n_steps < 1 || n_steps > (1 << 24)) return fail(GEMB200_E_INVALID, "n_steps must be in [1, 2^24]");
-  if (references && h->n_ref == 0) return fail(GEMB200_E_INVALID, "a reference feed needs a configuration with reference slots (n_ref > 0)");
+  if (int rc = check_rollout(h, n_steps, references)) return rc;
   PsOut po{};
   po.sio = sens_io; po.sout = sens_out; po.np = n_p;
   for (int a = 0; a < n_p; ++a) po.slot[a] = slots[a];
@@ -1184,7 +1122,7 @@ int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const voi
   for (int s = 0; s < 8; ++s) po.raw[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
-                 1.0, nullptr, nullptr, &po);
+                 1.0, &po);
 }
 
 int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, void* obs_out, void* ref_out, void* reward_out,

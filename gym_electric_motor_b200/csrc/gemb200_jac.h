@@ -1,6 +1,6 @@
-// gemb200_jac.h — the rollout-Jacobian launch (gemb200_rollout_jacobians), the return-gradient launch and the parameter-sensitivity launch
-// as the host unit sees them.  The kernels live in gemb200_tangent.cuh and are instantiated per (motor family, real) in gemb200_jac_tu.cu,
-// gemb200_grad_tu.cu and gemb200_psens_tu.cu.
+// gemb200_jac.h — the tangent-rollout launches as the host unit sees them: rollout Jacobians (gemb200_rollout_jacobians), return gradients
+// and parameter sensitivities, one launch_tangent_f overload per output kind.  The kernels live in gemb200_tangent.cuh and are instantiated
+// per (kind, motor family, real) from gemb200_tangent_tu.cu.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -16,7 +16,7 @@ struct JacOut {
   int nu;  // caller-side action width (0: finite converter)
 };
 
-template <int FAM, typename real> cudaError_t launch_jac_f(bool finite, int nref, const StepParams<real>& p, const JacOut& jo, cudaStream_t st);
+template <int FAM, typename real> cudaError_t launch_tangent_f(bool finite, int nref, const StepParams<real>& p, const JacOut& jo, cudaStream_t st);
 
 // Where the return gradients of gemb200_rollout_return_grads go, and how the reward reads the state row.  ws: the caller's workspace
 // [K][N][W] (W = n_x (n_x + n_u) + n_x + n_u words: one [J_x | J_u | d(g^k r_k)/dx | d(g^k r_k)/da] row per env and step); grad_a [K][N][n_u];
@@ -33,7 +33,8 @@ struct GradOut {
   int8_t rw_base[kMaxState];
 };
 
-template <int FAM, typename real> cudaError_t launch_grad_f(int nref, const StepParams<real>& p, const GradOut& go, cudaStream_t st);
+// finite: ignored, return gradients cover continuous converters only (gemb200_rollout_return_grads refuses finite ones)
+template <int FAM, typename real> cudaError_t launch_tangent_f(bool finite, int nref, const StepParams<real>& p, const GradOut& go, cudaStream_t st);
 
 // Where the parameter sensitivities of gemb200_rollout_param_sens go, and with respect to what.  sio: S = d x / d theta [N][n_x][n_p], read
 // at the start of the launch and overwritten with its value after the last step; sout: S after every step [K][N][n_x][n_p], or NULL; slot[c]:
@@ -47,6 +48,6 @@ struct PsOut {
   double raw[kMaxDraw];
 };
 
-template <int FAM, typename real> cudaError_t launch_psens_f(bool finite, int nref, const StepParams<real>& p, const PsOut& po, cudaStream_t st);
+template <int FAM, typename real> cudaError_t launch_tangent_f(bool finite, int nref, const StepParams<real>& p, const PsOut& po, cudaStream_t st);
 
 }  // namespace gemb200

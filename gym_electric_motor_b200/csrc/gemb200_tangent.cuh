@@ -759,26 +759,11 @@ jacobian_kernel(const __grid_constant__ StepParams<real> p, const __grid_constan
   real x[NX], rv[NREF > 0 ? NREF : 1], rs[NREF > 0 ? NREF : 1];
   uint32_t rend[NREF > 0 ? NREF : 1];
   bool cold_dirty = mech;
-  if (active) {
-    if constexpr (NH > 0) load_words<NH, real>(p.st, i, n, hot);
-    load_words<NC, real>(p.stc, i, n, cold);
-    ang.set(p.init_ang);
-    if constexpr (F::EPS) ang.load(p.eps, i);
-    unpack_records<NX, NREF, real>(hot, cold, x, rv, rs, rend);
-  }
-  if constexpr (ENVP) {
-    Coef<real> kl;
-    load_coef<FAM, real>(p, active ? i : (unsigned)p.env_begin, mech != 0, kl);
-    jac_loop<FAM, FINITE, real, NREF, true>(p, jo, kl, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
-  } else {
-    jac_loop<FAM, FINITE, real, NREF, false>(p, jo, p.k, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
-  }
-  if (active) {
-    pack_records<NX, NREF, real>(hot, cold, x, rv, rs, rend);
-    if constexpr (NH > 0) store_words<NH, real>(p.st, i, n, hot);
-    if (cold_dirty) store_words<NC, real>(p.stc, i, n, cold);
-    if constexpr (F::EPS) ang.store(p.eps, i);
-  }
+  if (active) load_record<FAM, NREF, real>(p, i, n, hot, cold, ang, x, rv, rs, rend);
+  with_coef<FAM, ENVP>(p, i, active, mech, [&](CoefArg<real, ENVP> kc) {
+    jac_loop<FAM, FINITE, real, NREF, ENVP>(p, jo, kc, i, active, x, ang, rv, rs, rend, cold_dirty, rows, row, jrows, jrow, jstride, lane, stride);
+  });
+  if (active) store_record<FAM, NREF, real>(p, i, n, hot, cold, ang, x, rv, rs, rend, cold_dirty);
 }
 
 // The load counterpart of warp_store_jac: the warp's rows (width w words) from `src` (the warp's first env's row) into shared memory

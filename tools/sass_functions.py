@@ -1,9 +1,10 @@
 """Kernel-by-kernel SASS comparison of two builds of the library's translation units.
 
-    python tools/sass_functions.py OLD_OBJ_DIR NEW_OBJ_DIR [--skip-envp] [--objects GLOB]
+    python tools/sass_functions.py OLD_OBJ_DIR NEW_OBJ_DIR [--skip-envp] [--objects GLOB | --all]
 
 Splits `cuobjdump -sass` of every object matching GLOB (default step_f*.o, the step translation units; host.o is the host unit with the
-snapshot, RNG-identity, parameter-block, clock, peer and accessor kernels) by function (instruction addresses and the source-path
+snapshot, RNG-identity, parameter-block, clock, peer and accessor kernels; jac_f*.o, grad_f*.o and psens_f*.o are the tangent-rollout
+units; --all: every object of the build) by function (instruction addresses and the source-path
 identifier removed) and compares each kernel with the one of the same name in the other build.  --skip-envp leaves out the ENVP instantiations (per-env parameter blocks: the
 8th template argument of step_kernel / rollout_kernel), reset_kernel and the parameter draw they call, whose code a change to the per-env parameter path is expected to
 touch; every other kernel must then be identical.  Prints one line per differing or missing kernel and a summary; exit code 1 if any
@@ -53,7 +54,7 @@ def is_envp_or_reset(pretty):
 def main():
     old_dir, new_dir = sys.argv[1], sys.argv[2]
     skip = "--skip-envp" in sys.argv
-    pattern = sys.argv[sys.argv.index("--objects") + 1] if "--objects" in sys.argv else "step_f*.o"
+    pattern = "*.o" if "--all" in sys.argv else (sys.argv[sys.argv.index("--objects") + 1] if "--objects" in sys.argv else "step_f*.o")
     same = differ = skipped = 0
     for new_obj in sorted(glob.glob(os.path.join(new_dir, pattern))):
         old_obj = os.path.join(old_dir, os.path.basename(new_obj))
