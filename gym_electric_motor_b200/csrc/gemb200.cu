@@ -603,6 +603,7 @@ static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
   for (int r = 0; r < GEMB200_MAX_REF_ENTRIES; ++r) p->sw_cdf[r] = (real)c.ref_sw_cdf[r];
   p->any_wiener = h->any_wiener;
   p->ref_tau = (real)c.tau;
+  p->ref_tau_d = c.tau;
   for (int r = 0; r < GEMB200_MAX_REF_ENTRIES; ++r) {  // all parameter entries (switched sub-generators live beyond n_ref)
     p->ref_kind[r] = c.ref_kind[r]; p->ref_state[r] = c.ref_state[r];
     p->ref_const[r] = (real)c.ref_value[r];
@@ -610,6 +611,7 @@ static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
     p->ref_init_lo[r] = (real)c.ref_init_lo[r]; p->ref_init_span[r] = (real)(c.ref_init_hi[r] - c.ref_init_lo[r]);
     p->ref_amp_lo[r] = (real)c.ref_amp_lo[r]; p->ref_amp_span[r] = (real)(c.ref_amp_hi[r] - c.ref_amp_lo[r]);
     p->ref_freq_lo[r] = (real)c.ref_freq_lo[r]; p->ref_freq_span[r] = (real)(c.ref_freq_hi[r] - c.ref_freq_lo[r]);
+    p->ref_freq_lo_d[r] = c.ref_freq_lo[r]; p->ref_freq_span_d[r] = c.ref_freq_hi[r] - c.ref_freq_lo[r];
     p->ref_off_lo[r] = (real)c.ref_off_lo[r]; p->ref_off_hi[r] = (real)c.ref_off_hi[r];
     if (c.ref_kind[r] == GEMB200_REF_WIENER || c.ref_kind[r] == GEMB200_REF_LAPLACE) {
       p->ref_lsig_lo[r] = (real)std::log10(c.ref_sigma_lo[r]);

@@ -271,6 +271,10 @@ struct StepParams {
   real* ret_out;
   int32_t* ret_end;
   real discount;
+  // ---- periodic generators in the fp32 build (periodic_value; general instantiations only, never PLAIN): the frequency range and tau in
+  //      double, so that the phase f tau k + phase of a long sub-episode is formed and reduced in double (DESIGN §2 finding 13) ----
+  double ref_freq_lo_d[kMaxRefEntries], ref_freq_span_d[kMaxRefEntries];
+  double ref_tau_d;
 };
 constexpr int kRngIdWords = 8;
 

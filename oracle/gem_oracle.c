@@ -75,6 +75,7 @@ typedef struct gem_oracle {
   double tq0; /* SCIM torque factor */
   uint64_t gstep; /* id of the current API call (RNG counter) */
   uint64_t n_steps; /* step calls so far (dead-time ring position) */
+  int exact_grid; /* 0: the reference's time grid (t accumulates, h = fl(t + tau) - t); 1: the device's (gem_oracle_set_time_grid) */
   env_t* env;
 } gem_oracle;
 
@@ -513,8 +514,8 @@ static const int B6_SUBACTIONS[8][3] = {{2, 2, 2}, {2, 2, 1}, {2, 1, 2}, {2, 1, 
 
 /* converter.set_action: returns the number of switching segments (1..3) and their END times: the sorted unique switching times of the
  * sub-converters (FiniteMultiConverter.set_action :583-595) — {t+tau}, {t+t_il, t+tau}, or with two different interlocking times
- * {t+t_lo, t+t_hi, t+tau}. */
-static int conv_set_action(const gem_oracle* o, env_t* e, const double* act_f, const int32_t* act_i, double t, double* seg_end) {
+ * {t+t_lo, t+t_hi, t+tau}.  seg_off (may be NULL): the same ends as offsets from t, {tau}, {t_il, tau} or {t_lo, t_hi, tau}. */
+static int conv_set_action_off(const gem_oracle* o, env_t* e, const double* act_f, const int32_t* act_i, double t, double* seg_end, double* seg_off) {
   int sw[2] = {0, 0};
   int ai = 0, af = 0;
   for (int slot = 0; slot < 2; ++slot) {
@@ -551,12 +552,17 @@ static int conv_set_action(const gem_oracle* o, env_t* e, const double* act_f, c
     }
   }
   int nseg = 0;
-  const double t0 = t + il_slot(o, 0), t1 = t + il_slot(o, 1);
-  if (sw[0] && sw[1] && t0 != t1) { seg_end[nseg++] = fmin(t0, t1); seg_end[nseg++] = fmax(t0, t1); }
-  else if (sw[0]) seg_end[nseg++] = t0;
-  else if (sw[1]) seg_end[nseg++] = t1;
-  seg_end[nseg++] = t + o->cfg.tau;
+  const double il0 = il_slot(o, 0), il1 = il_slot(o, 1), t0 = t + il0, t1 = t + il1;
+  double off[3];
+  if (sw[0] && sw[1] && t0 != t1) { seg_end[nseg] = fmin(t0, t1); off[nseg++] = fmin(il0, il1); seg_end[nseg] = fmax(t0, t1); off[nseg++] = fmax(il0, il1); }
+  else if (sw[0]) { seg_end[nseg] = t0; off[nseg++] = il0; }
+  else if (sw[1]) { seg_end[nseg] = t1; off[nseg++] = il1; }
+  seg_end[nseg] = t + o->cfg.tau; off[nseg++] = o->cfg.tau;
+  if (seg_off) for (int j = 0; j < nseg; ++j) seg_off[j] = off[j];
   return nseg;
+}
+static int conv_set_action(const gem_oracle* o, env_t* e, const double* act_f, const int32_t* act_i, double t, double* seg_end) {
+  return conv_set_action_off(o, e, act_f, act_i, t, seg_end, NULL);
 }
 
 /* converter.convert(i_out, t) -> u_in (not yet multiplied by u_sup); i_out laid out per slot */
@@ -708,9 +714,11 @@ static void simulate(const gem_oracle* o, env_t* e, const double* act_f, const i
   double u_sup = c->u_sup; /* IdealVoltageSupply.get_voltage voltage_supplies.py:70-72 */
   double* y = e->ode;
   double i_in[6], u_in[6], u_solver[4];
-  double t0 = e->t;
-  double seg_end[3];
-  int nseg = conv_set_action(o, e, act_f, act_i, t0, seg_end);
+  /* exact grid: step k of the episode starts at k tau and its segments have the lengths of the offsets' differences, tau, til,
+   * tau - til and |til1 - til0| (computed in double like the device's seg_len); the reference's t accumulates instead */
+  double t0 = o->exact_grid ? (double)e->k * c->tau : e->t;
+  double seg_end[3], seg_off[3];
+  int nseg = conv_set_action_off(o, e, act_f, act_i, t0, seg_end, seg_off);
   double t_solver = t0;
   const double* gt = NULL; /* ExternalSpeedLoad: the tabulated profile restarts at every reset (e->k = steps since then) */
   if (c->load_kind == GEMB200_LOAD_EXT_SPEED) {
@@ -764,10 +772,26 @@ static void simulate(const gem_oracle* o, env_t* e, const double* act_f, const i
       } break;
       default: u_solver[0] = u_in[0]; u_solver[1] = u_in[1]; break;
     }
-    t_solver = integrate(o, y, t_solver, seg_end[seg], u_solver, gt); /* :513 */
+    if (o->exact_grid && c->solver_kind == GEMB200_SOLVER_EULER) {
+      integrate_euler(o, y, seg_off[seg] - (seg ? seg_off[seg - 1] : 0.0), c->solver_nsteps, u_solver, gt);
+      t_solver = t0 + seg_off[seg];
+    } else if (o->exact_grid && c->solver_kind == GEMB200_SOLVER_RK4) {
+      integrate_rk4(o, y, seg_off[seg] - (seg ? seg_off[seg - 1] : 0.0), c->solver_nsteps, u_solver, gt);
+      t_solver = t0 + seg_off[seg];
+    } else {
+      t_solver = integrate(o, y, t_solver, seg_end[seg], u_solver, gt); /* :513 */
+    }
   }
   e->t = t_solver;
   e->k += 1;
+  /* exact grid: the angle is kept in [-pi, pi) like the device's (fmod is exact); the reference's unwrapped float64 angle rounds at the
+   * ulp of its magnitude, ~5e-9 rad after 1e5 steps at p omega = 300 rad/s, more than the fp64 parity bar */
+  if (o->exact_grid && mk >= GEMB200_MOTOR_PMSM) {
+    double* eps_state = y + o->n_ode - 1;
+    *eps_state = fmod(*eps_state, 2 * M_PI);
+    if (*eps_state >= M_PI) *eps_state -= 2 * M_PI;
+    else if (*eps_state < -M_PI) *eps_state += 2 * M_PI;
+  }
   const double* lim = c->limits;
   double tq = torque(o, y + 1);
   int n = 0;
@@ -1389,6 +1413,15 @@ void gem_oracle_rollout(gem_oracle* o, const void* actions, int64_t set_stride_b
   if (nthreads > 1) pthread_barrier_destroy(&bar);
   free(th); free(jobs);
 }
+
+/* Jump the handle's clock: call_id = id of the last API call (the next reset / step draws with call_id + 1), n_steps = step calls so far
+ * (dead-time ring position, periodic sub-episode keys).  The device's equivalent is a checkpoint with a patched header; env state,
+ * sub-episodes and dead-time queues are left as they are, so a test resets after the jump. */
+void gem_oracle_set_clock(gem_oracle* o, uint64_t call_id, uint64_t n_steps) { o->gstep = call_id; o->n_steps = n_steps; }
+void gem_oracle_get_clock(const gem_oracle* o, uint64_t* call_id, uint64_t* n_steps) { *call_id = o->gstep; *n_steps = o->n_steps; }
+/* exact = 0: the reference's time grid (default); 1: the device's, step k of an episode over [k tau, (k + 1) tau] with its segment lengths
+ * precomputed (fixed-step solvers) and the AC supply evaluated at k tau (DESIGN §2 finding 12) */
+void gem_oracle_set_time_grid(gem_oracle* o, int exact) { o->exact_grid = exact != 0; }
 
 void gem_oracle_get_ode_state(const gem_oracle* o, double* out) {
   for (int64_t i = 0; i < o->cfg.n_envs; ++i) memcpy(out + i * o->n_ode, o->env[i].ode, sizeof(double) * o->n_ode);

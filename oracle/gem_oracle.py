@@ -61,6 +61,9 @@ def lib():
         _lib.gem_oracle_probe_reward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]
         _lib.gem_oracle_probe_reward.restype = C.c_double
         _lib.gem_oracle_probe_euler.argtypes = [C.c_int, C.c_void_p, C.c_double, C.c_double, C.c_void_p]
+        _lib.gem_oracle_set_clock.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64]
+        _lib.gem_oracle_get_clock.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        _lib.gem_oracle_set_time_grid.argtypes = [C.c_void_p, C.c_int]
         _lib.gem_oracle_periodic_block.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     return _lib
 
@@ -122,6 +125,19 @@ class Oracle:
         term = np.zeros(self.n, dtype=np.uint8)
         self._lib.gem_oracle_rollout(self._h, _p(pool), pool.strides[0], pool.shape[0], int(n_steps), _p(obs), _p(ref), _p(rew), _p(term), self.nthreads)
         return obs, ref, rew, term
+
+    def set_clock(self, call_id, n_steps):
+        """Jump to the clock (call id of the last API call, step calls so far) that VectorSim.clock() reports; reset afterwards."""
+        self._lib.gem_oracle_set_clock(self._h, int(call_id), int(n_steps))
+
+    def clock(self):
+        a, b = C.c_uint64(), C.c_uint64()
+        self._lib.gem_oracle_get_clock(self._h, C.byref(a), C.byref(b))
+        return int(a.value), int(b.value)
+
+    def set_time_grid(self, exact):
+        """exact=False (default): the reference's grid, t accumulated with t += tau; exact=True: the device's, step k over [k tau, (k+1) tau]."""
+        self._lib.gem_oracle_set_time_grid(self._h, 1 if exact else 0)
 
     def get_ode_state(self):
         out = np.zeros((self.n, self.n_ode))

@@ -724,7 +724,7 @@ def test_more_reference_generators_match_oracle(torch_cuda, oracle_lib, kinds, d
     ora = oracle_lib.Oracle(mk(K.F64), nthreads=8)
     _, o_ref = ora.reset()
     _, d_ref = dev.reset()
-    tol = 1e-9 if dtype == K.F64 else 2e-4
+    tol = 1e-9 if dtype == K.F64 else 1e-5  # fp32: the phase is formed in double (DESIGN §2 finding 13)
     bad = int((np.abs(d_ref - o_ref) > tol).sum())
     total = d_ref.size
     rng = np.random.default_rng(1)
