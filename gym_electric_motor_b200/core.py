@@ -215,15 +215,17 @@ class ElectricMotorEnvironment(_EnvBase):
         for callback in self._callbacks:
             getattr(callback, func_name)(*args)
 
-    def _filter(self, obs):
+    def _require_batched(self, name):
+        if self._scalar:
+            raise TypeError(f"{name}() needs a batched environment (num_envs=...)")
+
+    def _filter(self, obs, lead=0):
+        """the state-filter entries of obs: its state axis is 0 (SoA) or 1 (AoS), after `lead` leading step axes"""
         if self._filter_identity:
             return obs
-        import torch
-
         if self._filter_index is None:
             self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
-        dim = 0 if self._sim.soa else 1
-        return obs.index_select(dim, self._filter_index)
+        return obs.index_select((0 if self._sim.soa else 1) + lead, self._filter_index)
 
     # ------------------------------------------------------------------ gym API
     def reset(self, seed=None, options=None, mask=None, *_, **__):
@@ -285,18 +287,12 @@ class ElectricMotorEnvironment(_EnvBase):
         `set_reference(references[k]); step(actions[k])`.  The returned reference of step k is what that loop returns: for an External
         slot the value step k was scored against (the reset value on an env that was auto-reset in step k).  A policy that needs a preview
         reads it from `references` itself.  Wrong shape, dtype, device or K: ValueError."""
-        if self._scalar:
-            raise TypeError("rollout() needs a batched environment (num_envs=...)")
+        self._require_batched("rollout")
         sim = self._ensure_sim()
         obs, ref, reward, terminated = sim.rollout(actions, record_every) if references is None else sim.rollout(actions, record_every, references)
         k = int(actions.shape[0]) if hasattr(actions, "shape") else len(actions)
         self._physical_system._k += k
-        if not self._filter_identity:
-            if self._filter_index is None:
-                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
-            dim = (0 if sim.soa else 1) + (1 if record_every else 0)
-            obs = obs.index_select(dim, self._filter_index)
-        return (obs, ref), reward, terminated.view(torch.bool)
+        return (self._filter(obs, 1 if record_every else 0), ref), reward, terminated.view(torch.bool)
 
     def rollout_returns(self, actions, discount=1.0, references=None):
         """Score an action sequence: K steps with pre-computed actions [K, N, n_act] (SoA: [K, n_act, N]) in ONE kernel launch that hands
@@ -307,16 +303,11 @@ class ElectricMotorEnvironment(_EnvBase):
         (state, reference): the last step's outputs as `rollout(actions, record_every=0)` returns them, to bootstrap the envs with
         end_step == K.  The env ends in exactly the state of `rollout(actions, references=references)`.  discount: finite, in [0, 1].
         references: the reference feed of `rollout`.  Batched mode only; bad actions, discount or feed: ValueError before any launch."""
-        if self._scalar:
-            raise TypeError("rollout_returns() needs a batched environment (num_envs=...)")
+        self._require_batched("rollout_returns")
         sim = self._ensure_sim()
         ret, end, (obs, ref) = sim.rollout_returns(actions, discount, references)
         self._physical_system._k += int(actions.shape[0])
-        if not self._filter_identity:
-            if self._filter_index is None:
-                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
-            obs = obs.index_select(0 if sim.soa else 1, self._filter_index)
-        return ret, end, (obs, ref)
+        return ret, end, (self._filter(obs), ref)
 
     def rollout_jacobians(self, actions, references=None):
         """Linearise the plant along an action sequence: K steps with pre-computed actions [K, N, n_act] in ONE kernel launch that also
@@ -327,16 +318,11 @@ class ElectricMotorEnvironment(_EnvBase):
         the Jacobian of the physical step it took.  `calc_jacobian` does not switch this on or off.  Refused configurations (dead time, RC
         supply, dq actions on the observer angle, SoA): NotImplementedError (DESIGN.md §7).
         Batched mode only; bad actions or feed: ValueError before any launch."""
-        if self._scalar:
-            raise TypeError("rollout_jacobians() needs a batched environment (num_envs=...)")
+        self._require_batched("rollout_jacobians")
         sim = self._ensure_sim()
         (jx, ju), (obs, ref, reward, terminated) = sim.rollout_jacobians(actions, references)
         self._physical_system._k += int(actions.shape[0])
-        if not self._filter_identity:
-            if self._filter_index is None:
-                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
-            obs = obs.index_select(2, self._filter_index)
-        return (jx, ju), ((obs, ref), reward, terminated.view(torch.bool))
+        return (jx, ju), ((self._filter(obs, 1), ref), reward, terminated.view(torch.bool))
 
     def rollout_return_grads(self, actions, discount=1.0, references=None, value_grad=None):
         """Score an action sequence and differentiate the score: `rollout_returns` plus, from the same launch, grad_a [K, N, n_u] =
@@ -349,16 +335,11 @@ class ElectricMotorEnvironment(_EnvBase):
         perturbed sequence would hit (DESIGN.md §7).  Refused configurations (those of `rollout_jacobians`, finite converters, a reward on
         an entry a state wrapper appends): NotImplementedError.  Batched mode only; bad actions, discount, feed or value_grad: ValueError
         before any launch."""
-        if self._scalar:
-            raise TypeError("rollout_return_grads() needs a batched environment (num_envs=...)")
+        self._require_batched("rollout_return_grads")
         sim = self._ensure_sim()
         ret, end, (obs, ref), ga, gx = sim.rollout_return_grads(actions, discount, references, value_grad)
         self._physical_system._k += int(actions.shape[0])
-        if not self._filter_identity:
-            if self._filter_index is None:
-                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
-            obs = obs.index_select(1, self._filter_index)
-        return ret, end, (obs, ref), ga, gx
+        return ret, end, (self._filter(obs), ref), ga, gx
 
     def differentiable_returns(self, actions, discount=1.0, references=None):
         """`rollout_returns(actions, discount, references)[0]` as a torch autograd function of `actions`: the forward pass runs ONE
@@ -366,8 +347,7 @@ class ElectricMotorEnvironment(_EnvBase):
         grad_output[None, :, None] * grad_a.  So an action sequence that is an `nn.Parameter`, or the output of a policy, can be optimised
         with a torch optimiser.  Every call starts from the env's current state: to evaluate the same start again, branch the envs first
         (`snapshot_envs`) and put them back with `restore_envs(..., rng="source")` before the next call."""
-        if self._scalar:
-            raise TypeError("differentiable_returns() needs a batched environment (num_envs=...)")
+        self._require_batched("differentiable_returns")
         if not isinstance(actions, torch.Tensor):
             raise ValueError(f"actions must be a torch tensor, got {type(actions).__name__}")
         return _DifferentiableReturns.apply(actions, self, discount, references)
@@ -407,19 +387,14 @@ class ElectricMotorEnvironment(_EnvBase):
         of the physical step it took; an env auto-reset in it carries S = 0 from there.  Refused configurations (those of
         `rollout_jacobians`) and parameter draws at resets: NotImplementedError (DESIGN.md §7).  Batched mode only; bad actions, feed or
         sens0: ValueError before any launch."""
-        if self._scalar:
-            raise TypeError("rollout_param_sensitivities() needs a batched environment (num_envs=...)")
+        self._require_batched("rollout_param_sensitivities")
         slots = self.param_slots(params)
         sim = self._ensure_sim()
         if getattr(self, "_randomized_names", ()):
             raise NotImplementedError("parameter sensitivities are refused while parameter draws at resets are on (DESIGN.md §7)")
         (so, sl), (obs, ref, reward, terminated) = sim.rollout_param_sens(actions, slots, references, sens0, record)
         self._physical_system._k += int(actions.shape[0])
-        if not self._filter_identity:
-            if self._filter_index is None:
-                self._filter_index = torch.as_tensor(self.state_filter, device=obs.device)
-            obs = obs.index_select(2, self._filter_index)
-        return (so, sl), ((obs, ref), reward, terminated.view(torch.bool))
+        return (so, sl), ((self._filter(obs, 1), ref), reward, terminated.view(torch.bool))
 
     def capture_steps(self, policy, n_steps, record=False, warmup=1, references=None):
         """`n_steps` closed-loop steps — action = policy(state, reference); env.step(action) — captured ONCE in a CUDA graph (graph.py);
@@ -442,8 +417,7 @@ class ElectricMotorEnvironment(_EnvBase):
         normalisation stay those of the env.  `set_env_parameters()` without arguments returns to the shared parameters.  Pole pairs `p` may
         be named only with the env's own value (ValueError otherwise: the angle increments are prepared per handle); the flux limits of an
         induction motor's random initial states and the FluxObserver's constants stay those of the env's nominal motor (DESIGN.md §7)."""
-        if self._scalar:
-            raise TypeError("set_env_parameters() needs a batched environment (num_envs=...)")
+        self._require_batched("set_env_parameters")
         sim = self._ensure_sim()
         if not motor_parameter and not load_parameter:
             sim.set_env_params(None, None)
@@ -475,8 +449,7 @@ class ElectricMotorEnvironment(_EnvBase):
         (ValueError); nor, for induction motors with random initial states, the parameters of their flux limits (NotImplementedError).
         Needs the row-per-env (AoS) layout (ValueError).  While draws are on, checkpoints are refused, and so are snapshots and restores
         unless they carry the parameters (`snapshot_envs(..., params=True)`, `restore_envs(..., params="source")`; DESIGN.md §7)."""
-        if self._scalar:
-            raise TypeError("randomize_env_parameters() needs a batched environment (num_envs=...)")
+        self._require_batched("randomize_env_parameters")
         from .randomization import encode_distributions
 
         cfg = self._sim.cfg if self._sim is not None else self.build_config()
@@ -505,8 +478,7 @@ class ElectricMotorEnvironment(_EnvBase):
         takes their physical parameters (`snap.params`, float64 [m, 24] in the slot order of `_cabi.MP_*`, then `MAX_MOTOR_PARAM + LP_*`:
         per-env values, drawn or set from the host, or the env's own), which `restore_envs(..., params="source")` hands on; it is allowed
         while parameters are drawn per reset and needs the row-per-env layout (ValueError).  Batched mode only."""
-        if self._scalar:
-            raise TypeError("snapshot_envs() needs a batched environment (num_envs=...)")
+        self._require_batched("snapshot_envs")
         from .snapshot import check_host_index, check_params_layout
 
         sim = self._ensure_sim()
@@ -520,8 +492,7 @@ class ElectricMotorEnvironment(_EnvBase):
         """Every env draws its own random numbers again (drops the identities adopted with `restore_envs(..., rng="source")`); afterwards
         the envs draw exactly what they would have drawn had they never adopted one, and the env runs its shared-coefficient kernels again
         unless it has per-env parameters of its own.  Batched mode only."""
-        if self._scalar:
-            raise TypeError("clear_rng_identities() needs a batched environment (num_envs=...)")
+        self._require_batched("clear_rng_identities")
         self._ensure_sim().clear_rng_ids()
 
     def restore_envs(self, snapshot, idx=None, rows=None, rng="own", params="own"):
@@ -540,8 +511,7 @@ class ElectricMotorEnvironment(_EnvBase):
         is what branching domain-randomised envs needs, and it is allowed while parameters are drawn per reset.  The values of
         `snapshot.params` are used as given, so an edited copy restores an ensemble of plants; the pole-pair slot is ignored, and pole pairs
         differing from this env's raise ValueError.  Afterwards the env runs per-env parameter blocks (DESIGN.md §7)."""
-        if self._scalar:
-            raise TypeError("restore_envs() needs a batched environment (num_envs=...)")
+        self._require_batched("restore_envs")
         from .snapshot import check_host_index, check_layout, check_params_mode, check_rng_mode
 
         sim = self._ensure_sim()

@@ -59,6 +59,10 @@ class VectorSim:
     def _shape(self, k):
         return (k, self.n) if self.soa else (self.n, k)
 
+    def _ref_ptr(self, ref):
+        """the reference output of a launch: NULL without reference slots"""
+        return _ptr(ref) if self.n_ref else None
+
     def _alloc_outputs(self):
         if self._reuse and self._out is not None:
             return self._out
@@ -72,6 +76,15 @@ class VectorSim:
         if self._reuse:
             self._out = out
         return out
+
+    def _alloc_stacked(self, s):
+        """(obs, ref, reward, terminated) of s recorded steps, stacked on a leading axis"""
+        return (
+            torch.empty((s,) + self._shape(self.n_state), dtype=self.dtype, device=self.device),
+            torch.empty((s,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device),
+            torch.empty((s, self.n), dtype=self.dtype, device=self.device),
+            torch.empty((s, self.n), dtype=torch.uint8, device=self.device),
+        )
 
     def bind_outputs(self, obs, ref, reward, terminated):
         """Let the step / reset launches write into caller-owned tensors (e.g. the sections of a packed all-gather buffer,
@@ -102,7 +115,7 @@ class VectorSim:
         m = None
         if mask is not None:
             m = torch.as_tensor(mask, device=self.device).to(torch.uint8).contiguous()
-        K.check(self._lib.gemb200_reset(self._h, _ptr(m), _ptr(obs), _ptr(ref) if self.n_ref else None, self._stream()), "gemb200_reset")
+        K.check(self._lib.gemb200_reset(self._h, _ptr(m), _ptr(obs), self._ref_ptr(ref), self._stream()), "gemb200_reset")
         return obs, ref
 
     def reseed(self, seed):
@@ -180,7 +193,9 @@ class VectorSim:
     def _as_feed(self, references, k):
         """check a reference feed of k steps: a contiguous device tensor of the handle's dtype, shaped [k, N, n_ref] (SoA: [k, n_ref, N]);
         k = None: one step, [N, n_ref] (SoA: [n_ref, N]).  Nothing is converted: a feed is read in place by the launch (and by every replay
-        of a captured one)."""
+        of a captured one).  No feed (None) stays None."""
+        if references is None:
+            return None
         if not self.n_ref:
             raise ValueError("a reference feed needs reference slots: this configuration has n_ref == 0")
         shape = self._shape(self.n_ref) if k is None else (int(k),) + self._shape(self.n_ref)
@@ -202,65 +217,48 @@ class VectorSim:
             r = self._as_feed(reference, None)
             a = self._as_action(action)
             obs, ref, rew, term = out = self._alloc_outputs()
-            K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(a), _ptr(r), 1, 0, _ptr(obs), _ptr(ref), _ptr(rew), _ptr(term),
-                                                         self._stream()), "gemb200_rollout_record_ref")
+            self.rollout_into(a, 1, 0, obs, ref, rew, term, r[None])  # the K = 1 feed is a view: a captured step reads the caller's tensor
             return out
         a = self._as_action(action)
         out = self._alloc_outputs()
         if self._reuse:
             if getattr(self, "_out_ptrs", None) is None:
                 obs, ref, rew, term = out
-                self._out_ptrs = (_ptr(obs), _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term))
+                self._out_ptrs = (_ptr(obs), self._ref_ptr(ref), _ptr(rew), _ptr(term))
             po, pr, pw, pt = self._out_ptrs
         else:
             obs, ref, rew, term = out
-            po, pr, pw, pt = _ptr(obs), _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term)
+            po, pr, pw, pt = _ptr(obs), self._ref_ptr(ref), _ptr(rew), _ptr(term)
         rc = self._lib.gemb200_step(self._h, a.data_ptr(), po, pr, pw, pt, torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             K.check(rc, "gemb200_step")
         return out
 
     def rollout(self, actions, record_every=0, references=None):
-        """K open-loop env.step calls fused into ONE launch (gemb200_rollout_record): every env's record stays in registers for all K
+        """K open-loop env.step calls fused into ONE launch (gemb200_rollout_record_ref): every env's record stays in registers for all K
         steps; bit-identical to K calls of `step`.  actions: [K, N, n_act] (SoA layout: [K, n_act, N]).
         record_every = 0 -> the outputs of the last step (obs, ref, reward, terminated), shapes as `step`;
         record_every = m >= 1 -> the outputs of steps m, 2m, ... stacked on a leading axis of length K // m (m = 1: full trajectory).
-        references ([K, N, n_ref], SoA [K, n_ref, N], the handle's dtype, on the device; gemb200_rollout_record_ref): step k first
-        overwrites the stored value of EVERY reference slot with references[k] — the same as K iterations of
-        `set_reference(references[k]); step(actions[k])`."""
+        references ([K, N, n_ref], SoA [K, n_ref, N], the handle's dtype, on the device; None: no feed): step k first overwrites the stored
+        value of EVERY reference slot with references[k] — the same as K iterations of `set_reference(references[k]); step(actions[k])`."""
         a = actions if (isinstance(actions, torch.Tensor) and actions.dtype == self.act_dtype and actions.device == self.device and actions.is_contiguous()) \
             else torch.as_tensor(actions, device=self.device).to(self.act_dtype).contiguous()
         k = int(a.shape[0])
         if a.numel() != k * self.n * self.n_act:
             raise ValueError(f"actions must hold K x {self.n} x {self.n_act} values")
-        r = None if references is None else self._as_feed(references, k)
+        r = self._as_feed(references, k)
         m = int(record_every)
-        if m == 0:
-            obs, ref, rew, term = self._alloc_outputs()
-        else:
-            s = k // m
-            obs = torch.empty((s,) + self._shape(self.n_state), dtype=self.dtype, device=self.device)
-            ref = torch.empty((s,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device)
-            rew = torch.empty((s, self.n), dtype=self.dtype, device=self.device)
-            term = torch.empty((s, self.n), dtype=torch.uint8, device=self.device)
-        if r is None:
-            K.check(self._lib.gemb200_rollout_record(self._h, _ptr(a), k, m, _ptr(obs), _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term),
-                                                     self._stream()), "gemb200_rollout_record")
-        else:
-            K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(a), _ptr(r), k, m, _ptr(obs), _ptr(ref), _ptr(rew), _ptr(term), self._stream()),
-                    "gemb200_rollout_record_ref")
+        obs, ref, rew, term = self._alloc_outputs() if m == 0 else self._alloc_stacked(k // m)
+        self.rollout_into(a, k, m, obs, ref, rew, term, r)
         return obs, ref, rew, term
 
     def rollout_into(self, actions, n_steps, record_every, obs, ref, rew, term, references=None):
         """Raw variant for benchmarking: caller-owned output tensors (any may be None), no allocation, no conversion.  references: the
         reference feed of `rollout`, checked like there."""
-        if references is None:
-            K.check(self._lib.gemb200_rollout_record(self._h, _ptr(actions), int(n_steps), int(record_every), _ptr(obs), _ptr(ref) if self.n_ref else None,
-                                                     _ptr(rew), _ptr(term), self._stream()), "gemb200_rollout_record")
-            return
         r = self._as_feed(references, n_steps)
-        K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(actions), _ptr(r), int(n_steps), int(record_every), _ptr(obs), _ptr(ref),
-                                                     _ptr(rew), _ptr(term), self._stream()), "gemb200_rollout_record_ref")
+        K.check(self._lib.gemb200_rollout_record_ref(self._h, _ptr(actions), _ptr(r), int(n_steps), int(record_every), _ptr(obs), self._ref_ptr(ref),
+                                                     _ptr(rew), _ptr(term), self._stream()),
+                "gemb200_rollout_record" if r is None else "gemb200_rollout_record_ref")  # without a feed this is gemb200_rollout_record
 
     def _as_actions(self, actions):
         """check the actions of a fused launch: a contiguous device tensor of the action dtype, shaped [K, N, n_act] (SoA: [K, n_act, N])
@@ -294,30 +292,34 @@ class VectorSim:
         a = self._as_actions(actions)
         k = int(a.shape[0])
         g = self._as_discount(discount)
-        r = None if references is None else self._as_feed(references, k)
+        r = self._as_feed(references, k)
         obs, ref, _, _ = self._alloc_outputs()
         ret = torch.empty(self.n, dtype=self.dtype, device=self.device)
         end = torch.empty(self.n, dtype=torch.int32, device=self.device)
-        K.check(self._lib.gemb200_rollout_returns(self._h, _ptr(a), _ptr(r), k, g, _ptr(ret), _ptr(end), _ptr(obs), _ptr(ref) if self.n_ref else None,
-                                                  self._stream()), "gemb200_rollout_returns")
+        self.rollout_returns_into(a, k, g, ret, end, obs, ref, r)
         return ret, end, (obs, ref)
 
     def rollout_returns_into(self, actions, n_steps, discount, ret, end=None, obs=None, ref=None, references=None):
         """Raw variant of `rollout_returns` for benchmarking: caller-owned outputs (all but `ret` may be None), no allocation, no
         conversion.  The discount and the reference feed are checked like there."""
         g = self._as_discount(discount)
-        r = None if references is None else self._as_feed(references, n_steps)
+        r = self._as_feed(references, n_steps)
         K.check(self._lib.gemb200_rollout_returns(self._h, _ptr(actions), _ptr(r), int(n_steps), g, _ptr(ret), _ptr(end), _ptr(obs),
-                                                  _ptr(ref) if self.n_ref else None, self._stream()), "gemb200_rollout_returns")
+                                                  self._ref_ptr(ref), self._stream()), "gemb200_rollout_returns")
+
+    def _query_dims(self, query, n_out, *args):
+        """n_out int32 results of the configuration query `query` (no handle, no launch); NotImplementedError with the library's message
+        for a configuration the launch refuses"""
+        lib = K.load_library()
+        out = [C.c_int32() for _ in range(n_out)]
+        if getattr(lib, query)(C.byref(self.cfg), *args, *[C.byref(x) for x in out]):
+            raise NotImplementedError(lib.gemb200_last_error().decode())
+        return tuple(x.value for x in out)
 
     def jacobian_dims(self):
         """(n_x, n_u) of `rollout_jacobians`: n_x = n_ode, n_u = n_act (0 for finite converters).  NotImplementedError for a configuration the
         launch refuses (DESIGN.md §7)."""
-        lib = K.load_library()  # a configuration query: no handle, no launch
-        nx, nu = C.c_int32(), C.c_int32()
-        if lib.gemb200_query_jacobian_dims(C.byref(self.cfg), C.byref(nx), C.byref(nu)):
-            raise NotImplementedError(lib.gemb200_last_error().decode())
-        return nx.value, nu.value
+        return self._query_dims("gemb200_query_jacobian_dims", 2)
 
     def rollout_jacobians(self, actions, references=None):
         """K open-loop steps in ONE launch that also linearise the plant (gemb200_rollout_jacobians).  Returns ((jac_x, jac_u), (obs, ref, rew,
@@ -328,43 +330,33 @@ class VectorSim:
         nx, nu = self.jacobian_dims()
         a = self._as_actions(actions)
         k = int(a.shape[0])
-        r = None if references is None else self._as_feed(references, k)
+        r = self._as_feed(references, k)
         jx = torch.empty((k, self.n, nx, nx), dtype=self.dtype, device=self.device)
         ju = torch.empty((k, self.n, nx, nu), dtype=self.dtype, device=self.device) if nu else None
-        obs = torch.empty((k,) + self._shape(self.n_state), dtype=self.dtype, device=self.device)
-        ref = torch.empty((k,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device)
-        rew = torch.empty((k, self.n), dtype=self.dtype, device=self.device)
-        term = torch.empty((k, self.n), dtype=torch.uint8, device=self.device)
+        obs, ref, rew, term = self._alloc_stacked(k)
         self.rollout_jacobians_into(a, k, jx, ju, obs, ref, rew, term, r)
         return (jx, ju), (obs, ref, rew, term)
 
     def rollout_jacobians_into(self, actions, n_steps, jac_x, jac_u=None, obs=None, ref=None, rew=None, term=None, references=None):
         """Raw variant of `rollout_jacobians` for benchmarking: caller-owned outputs (all but `jac_x` may be None), no allocation, no
         conversion.  The reference feed is checked like there."""
-        r = None if references is None else self._as_feed(references, n_steps)
+        r = self._as_feed(references, n_steps)
         K.check(self._lib.gemb200_rollout_jacobians(self._h, _ptr(actions), _ptr(r), int(n_steps), _ptr(jac_x), _ptr(jac_u), _ptr(obs),
-                                                    _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term), self._stream()),
+                                                    self._ref_ptr(ref), _ptr(rew), _ptr(term), self._stream()),
                 "gemb200_rollout_jacobians")
 
     def return_grad_dims(self):
         """(n_x, n_u, ws_words) of `rollout_return_grads`: n_x = n_ode, n_u = n_act, ws_words = n_x (n_x + n_u) + n_x + n_u, the workspace
         words per env and step.  NotImplementedError for a configuration the launch refuses (DESIGN.md §7)."""
-        lib = K.load_library()  # a configuration query: no handle, no launch
-        nx, nu, ww = C.c_int32(), C.c_int32(), C.c_int32()
-        if lib.gemb200_query_return_grad_dims(C.byref(self.cfg), C.byref(nx), C.byref(nu), C.byref(ww)):
-            raise NotImplementedError(lib.gemb200_last_error().decode())
-        return nx.value, nu.value, ww.value
+        return self._query_dims("gemb200_query_return_grad_dims", 3)
 
-    def _as_value_grad(self, value_grad, nx):
-        if value_grad is None:
-            return None
-        shape = (self.n, nx)
-        if (not isinstance(value_grad, torch.Tensor) or value_grad.dtype != self.dtype or value_grad.device != self.device
-                or tuple(value_grad.shape) != shape or not value_grad.is_contiguous()):
-            got = (f"{tuple(value_grad.shape)} {value_grad.dtype} on {value_grad.device}" if isinstance(value_grad, torch.Tensor)
-                   else type(value_grad).__name__)
-            raise ValueError(f"value_grad must be a contiguous [{self.n}, {nx}] {self.dtype} tensor on {self.device}, got {got}")
-        return value_grad
+    def _as_tensor(self, t, name, shape):
+        """check `t` (None stays None): a contiguous tensor of `shape` in the handle's dtype on its device.  Nothing is converted."""
+        if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != self.dtype or t.device != self.device or tuple(t.shape) != shape
+                              or not t.is_contiguous()):
+            got = f"{tuple(t.shape)} {t.dtype} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"{name} must be a contiguous [{', '.join(map(str, shape))}] {self.dtype} tensor on {self.device}, got {got}")
+        return t
 
     def rollout_return_grads(self, actions, discount=1.0, references=None, value_grad=None):
         """`rollout_returns` with the gradients of the returns (gemb200_rollout_return_grads), in ONE launch.  Returns (returns, end_step,
@@ -378,8 +370,8 @@ class VectorSim:
         a = self._as_actions(actions)
         k = int(a.shape[0])
         g = self._as_discount(discount)
-        r = None if references is None else self._as_feed(references, k)
-        vg = self._as_value_grad(value_grad, nx)
+        r = self._as_feed(references, k)
+        vg = self._as_tensor(value_grad, "value_grad", (self.n, nx))
         obs, ref, _, _ = self._alloc_outputs()
         ret = torch.empty(self.n, dtype=self.dtype, device=self.device)
         end = torch.empty(self.n, dtype=torch.int32, device=self.device)
@@ -395,10 +387,10 @@ class VectorSim:
         n_steps * N * ws_words elements of the handle's dtype; `end`, `obs`, `ref` and `value_grad` may be None), no allocation, no
         conversion.  The discount and the reference feed are checked like there."""
         g = self._as_discount(discount)
-        r = None if references is None else self._as_feed(references, n_steps)
+        r = self._as_feed(references, n_steps)
         K.check(self._lib.gemb200_rollout_return_grads(self._h, _ptr(actions), _ptr(r), int(n_steps), g, _ptr(value_grad), _ptr(workspace),
                                                        workspace.numel() * workspace.element_size(), _ptr(ret), _ptr(end), _ptr(grad_a),
-                                                       _ptr(grad_x0), _ptr(obs), _ptr(ref) if self.n_ref else None, self._stream()),
+                                                       _ptr(grad_x0), _ptr(obs), self._ref_ptr(ref), self._stream()),
                 "gemb200_rollout_return_grads")
 
     @staticmethod
@@ -409,12 +401,8 @@ class VectorSim:
     def param_sens_dims(self, slots):
         """n_x of `rollout_param_sens` for the parameter slots `slots` (GEMB200_MP_* / GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_*): n_ode.
         NotImplementedError for a refused configuration or slot list (DESIGN.md §7)."""
-        lib = K.load_library()  # a configuration query: no handle, no launch
         arr, n_p = self._slot_array(slots)
-        nx = C.c_int32()
-        if lib.gemb200_query_param_sens_dims(C.byref(self.cfg), n_p, arr, C.byref(nx)):
-            raise NotImplementedError(lib.gemb200_last_error().decode())
-        return nx.value
+        return self._query_dims("gemb200_query_param_sens_dims", 1, n_p, arr)[0]
 
     def coef_tangents(self, slots, motor_param=None, load_param=None):
         """d (coefficient block) / d theta for the slots at a parameter row (the configuration's when None): float64 [n_p, 30] in the word
@@ -428,14 +416,6 @@ class VectorSim:
                                           out.ctypes.data), "gemb200_coef_tangents")
         return out
 
-    def _as_sens(self, sens, nx, n_p):
-        shape = (self.n, nx, n_p)
-        if (not isinstance(sens, torch.Tensor) or sens.dtype != self.dtype or sens.device != self.device or tuple(sens.shape) != shape
-                or not sens.is_contiguous()):
-            got = f"{tuple(sens.shape)} {sens.dtype} on {sens.device}" if isinstance(sens, torch.Tensor) else type(sens).__name__
-            raise ValueError(f"sens0 must be a contiguous [{self.n}, {nx}, {n_p}] {self.dtype} tensor on {self.device}, got {got}")
-        return sens
-
     def rollout_param_sens(self, actions, slots, references=None, sens0=None, record=True):
         """K open-loop steps in ONE launch that also carry the parameter sensitivities S = d x / d theta (gemb200_rollout_param_sens).
         Returns ((sens, sens_last), (obs, ref, rew, term)): sens [K, N, n_x, n_p] = d x_{k+1} / d theta after every step (None when
@@ -447,24 +427,21 @@ class VectorSim:
         n_p = len(slots)
         a = self._as_actions(actions)
         k = int(a.shape[0])
-        r = None if references is None else self._as_feed(references, k)
+        r = self._as_feed(references, k)
         sio = (torch.zeros((self.n, nx, n_p), dtype=self.dtype, device=self.device) if sens0 is None
-               else self._as_sens(sens0, nx, n_p).clone())
+               else self._as_tensor(sens0, "sens0", (self.n, nx, n_p)).clone())
         so = torch.empty((k, self.n, nx, n_p), dtype=self.dtype, device=self.device) if record else None
-        obs = torch.empty((k,) + self._shape(self.n_state), dtype=self.dtype, device=self.device)
-        ref = torch.empty((k,) + self._shape(self.n_ref), dtype=self.dtype, device=self.device)
-        rew = torch.empty((k, self.n), dtype=self.dtype, device=self.device)
-        term = torch.empty((k, self.n), dtype=torch.uint8, device=self.device)
+        obs, ref, rew, term = self._alloc_stacked(k)
         self.rollout_param_sens_into(a, k, slots, sio, so, obs, ref, rew, term, r)
         return (so, sio), (obs, ref, rew, term)
 
     def rollout_param_sens_into(self, actions, n_steps, slots, sens_io, sens_out=None, obs=None, ref=None, rew=None, term=None, references=None):
         """Raw variant of `rollout_param_sens` for benchmarking: caller-owned outputs (all but `sens_io` may be None; sens_io is read as S_0
         and overwritten with S_K), no allocation, no conversion.  The reference feed is checked like there."""
-        r = None if references is None else self._as_feed(references, n_steps)
+        r = self._as_feed(references, n_steps)
         arr, n_p = self._slot_array(slots)
         K.check(self._lib.gemb200_rollout_param_sens(self._h, _ptr(actions), _ptr(r), int(n_steps), n_p, arr, _ptr(sens_io), _ptr(sens_out), _ptr(obs),
-                                                     _ptr(ref) if self.n_ref else None, _ptr(rew), _ptr(term), self._stream()),
+                                                     self._ref_ptr(ref), _ptr(rew), _ptr(term), self._stream()),
                 "gemb200_rollout_param_sens")
 
     # ------------------------------------------------------------------ host-buffer API (numpy)
