@@ -47,32 +47,29 @@ def is_stale(out=OUT):
     return any(os.path.getmtime(d) > t for d in HEADERS + SOURCES if os.path.exists(d))
 
 
-def _units(only=None):
+def _units():
     units = [("host", SOURCES[0], LINEINFO)]
     for fam in FAMILIES:
         for real in REALS:
-            if only and (fam, real) not in only:
-                continue
             units.append((f"step_f{fam}_{real}", SOURCES[1], [f"-DGEMB200_TU_FAM={fam}", f"-DGEMB200_TU_REAL={real}"] + (LINEINFO if real == "float" else [])))
-    if not only:  # the tangent-rollout kernels: one unit per kind x family x real, like the step kernels
-        for prefix, out in TANGENT_KINDS:
-            for fam in FAMILIES:
-                for real in REALS:
-                    units.append((f"{prefix}_f{fam}_{real}", SOURCES[2], [f"-DGEMB200_TAN_OUT={out}", f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
+    # the tangent-rollout kernels: one unit per kind x family x real, like the step kernels
+    for prefix, out in TANGENT_KINDS:
+        for fam in FAMILIES:
+            for real in REALS:
+                units.append((f"{prefix}_f{fam}_{real}", SOURCES[2], [f"-DGEMB200_TAN_OUT={out}", f"-DGEMB200_JAC_FAM={fam}", f"-DGEMB200_JAC_REAL={real}"]))
     return units
 
 
-def build(force=False, verbose=False, out=OUT, defines=(), only=None, jobs=None):
-    """Compile and link.  `defines`/`only`/`out` are for experiment builds (tools/build_variants.py): extra -D flags, a subset of
-    (family, real) units — pass -DGEMB200_ONLY_FAM=<family> with only={(family, "float")} so that the host code does not reference
-    the missing units (otherwise the library fails to LOAD, on purpose: no silent holes) — and another output path."""
+def build(force=False, verbose=False, out=OUT, jobs=None):
+    """Compile and link into `out`.  Another output path gives a second library with its own object directory, e.g. the build of
+    another commit to compare against (GEMB200_LIB selects the library that _cabi loads); `jobs` caps the parallel nvcc processes."""
     if not force and not is_stale(out):
         return out
-    tag = hashlib.sha1(("|".join(defines) + "|" + os.path.abspath(out)).encode()).hexdigest()[:10]
+    tag = hashlib.sha1(("|" + os.path.abspath(out)).encode()).hexdigest()[:10]
     obj_dir = os.path.join(OBJ_DIR, tag)
     os.makedirs(obj_dir, exist_ok=True)
     nvcc = nvcc_path()
-    extra = list(defines) + (["-Xptxas", "-v"] if verbose else [])
+    extra = ["-Xptxas", "-v"] if verbose else []
 
     def compile_one(unit):
         name, src, flags = unit
@@ -81,7 +78,7 @@ def build(force=False, verbose=False, out=OUT, defines=(), only=None, jobs=None)
         res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         return obj, res
 
-    units = _units(only)
+    units = _units()
     with ThreadPoolExecutor(max_workers=jobs or min(len(units), os.cpu_count() or 4)) as ex:
         results = list(ex.map(compile_one, units))
     objs = []

@@ -556,11 +556,10 @@ static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
     const char* off = std::getenv("GEMB200_NO_PLAIN");
     plain_shape = plain && !(off && off[0] == '1');
   }
-  {  // L2 prefetch distance: one wave of resident threads (SMs x blocks/SM x block size); GEMB200_PF_DIST overrides (0 = off)
+  {  // L2 prefetch distance: one wave of resident threads (SMs x blocks/SM x block size)
     int sms = 132;  // H100 SXM; the attribute query below gives the real count
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c.device);
-    p->pf_dist = sms * 4 * GEMB200_BLOCK;  // one wave of 4 blocks per SM
-    if (const char* e = std::getenv("GEMB200_PF_DIST")) p->pf_dist = std::atoi(e);
+    p->pf_dist = sms * 4 * kBlock;  // one wave of 4 blocks per SM
   }
   p->ext_tab = static_cast<const real*>(h->d_ext);
   p->ext_len = c.ext_speed_len;
@@ -625,15 +624,9 @@ static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
 // ----------------------------------------------------------------------------------------------------------------
 // kernel dispatch (the instantiations live in gemb200_step_tu.cu and gemb200_tangent_tu.cu, one TU per family x real and kind)
 // ----------------------------------------------------------------------------------------------------------------
-// launch(std::integral_constant<int, FAM>{}) for motor family fam.  GEMB200_ONLY_FAM=<family>: experiment builds (tools/build_variants.py
-// --only) that carry the fp32 step and reset kernels of ONE motor family and no tangent kernels (TANGENT: a tangent-rollout launch); every
-// other launch fails with cudaErrorInvalidValue instead of leaving unresolved symbols.  Never defined in the product build.
-template <bool TANGENT, typename real, typename L>
+// launch(std::integral_constant<int, FAM>{}) for motor family fam
+template <typename L>
 static cudaError_t for_family(int fam, L&& launch) {
-#ifdef GEMB200_ONLY_FAM
-  if constexpr (!TANGENT && std::is_same<real, float>::value) { if (fam == GEMB200_ONLY_FAM) return launch(std::integral_constant<int, GEMB200_ONLY_FAM>{}); }
-  return cudaErrorInvalidValue;
-#else
   switch (fam) {
     case kDC1: return launch(std::integral_constant<int, kDC1>{});
     case kDC2: return launch(std::integral_constant<int, kDC2>{});
@@ -643,7 +636,6 @@ static cudaError_t for_family(int fam, L&& launch) {
     case kDFIM: return launch(std::integral_constant<int, kDFIM>{});
   }
   return cudaErrorInvalidValue;
-#endif
 }
 
 template <typename real>
@@ -717,9 +709,9 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
     set_roll_strides(h, p);
     const bool finite = h->cfg.finite != 0;
     if constexpr (!std::is_void<TanOut>::value) {
-      if (tan) return for_family<true, real>(h->fam, [&](auto f) { return launch_tangent_f<decltype(f)::value, real>(finite, h->n_ref, p, *tan, st); });
+      if (tan) return for_family(h->fam, [&](auto f) { return launch_tangent_f<decltype(f)::value, real>(finite, h->n_ref, p, *tan, st); });
     }
-    return for_family<false, real>(h->fam, [&](auto f) { return launch_step_f<decltype(f)::value, real>(finite, h->n_ref, p, st); });
+    return for_family(h->fam, [&](auto f) { return launch_step_f<decltype(f)::value, real>(finite, h->n_ref, p, st); });
   });
   if (e != cudaSuccess) return fail(GEMB200_E_CUDA, std::string(roll > 0 ? "rollout launch: " : "step launch: ") + cudaGetErrorString(e));
   h->launches += 1;
@@ -737,7 +729,7 @@ static int do_reset(gemb200_handle* h, const uint8_t* mask, void* obs, void* ref
     p.clock_dev = dev_clock ? h->d_clock : nullptr;
     p.gstep_lo = (uint32_t)h->gstep; p.gstep_hi = (uint32_t)(h->gstep >> 32);
     p.reset_mask = mask; p.obs = (real*)obs; p.ref_out = (real*)ref; p.kstep = dev_clock ? 0u : (uint32_t)h->n_steps;
-    const cudaError_t le = for_family<false, real>(h->fam, [&](auto f) { return launch_reset_f<decltype(f)::value, real>(h->n_ref, p, st); });
+    const cudaError_t le = for_family(h->fam, [&](auto f) { return launch_reset_f<decltype(f)::value, real>(h->n_ref, p, st); });
     p.reset_mask = nullptr;
     return le;
   });
@@ -1410,8 +1402,7 @@ int gemb200_step_host(gemb200_handle* h, const void* action, void* obs_out, void
   // Row-per-env buffers are contiguous per env range, so a large batch is cut into chunks that flow through three
   // streams: the D2H of chunk c overlaps the H2D + launch of chunk c+1 (PCIe is full duplex).  One API call = one RNG id.
   const bool pipelined = h->cfg.layout == GEMB200_LAYOUT_AOS && n >= (size_t)1 << 16;
-  static const int chunks_env = [] { const char* e = std::getenv("GEMB200_HOST_CHUNKS"); return e ? std::atoi(e) : 0; }();  // experiment knob
-  const int nchunk = pipelined ? (chunks_env > 0 ? chunks_env : 4) : 1;  // PCIe D2H bound; 4 keeps the copy count low
+  const int nchunk = pipelined ? 4 : 1;  // PCIe D2H bound; 4 keeps the copy count low
   const size_t per = pipelined ? ((n / nchunk + 255) / 256) * 256 : n;
   bool first = true;
   for (int c = 0; c < nchunk; ++c) {

@@ -4,8 +4,6 @@
 // (family, real) pair is compiled in its own translation unit (gemb200_step_tu.cu with -DGEMB200_TU_FAM / -DGEMB200_TU_REAL) so that
 // the library builds in parallel.  gemb200.cu only sees the declarations below.
 #pragma once
-#include <cstdlib>
-
 #include "gemb200_kernels.cuh"
 
 namespace gemb200 {
@@ -16,14 +14,10 @@ template <int FAM, typename real> cudaError_t launch_step_f(bool finite, int nre
 template <int FAM, typename real> cudaError_t launch_reset_f(int nref, const StepParams<real>& p, cudaStream_t st);
 
 #ifdef GEMB200_TU_FAM
-constexpr int kBlock = GEMB200_BLOCK;
-
 // Block size of a launch: kBlock (128) threads, or — for batches too small to give every SM its share of 128-thread blocks — 64 or 32, so that
 // the blocks spread evenly (N = 65 536: 512 blocks of 128 threads are 3.46 per SM, i.e. a 4-vs-3 imbalance; 2048 blocks of 32 are 13.8).  The
-// kernels index with blockDim.x, so the choice is a launch parameter.  GEMB200_BLOCK_RT=<32|64|128> overrides (experiments).
+// kernels index with blockDim.x, so the choice is a launch parameter.
 static int pick_block(int range) {
-  static const int forced = [] { const char* e = std::getenv("GEMB200_BLOCK_RT"); return e ? std::atoi(e) : 0; }();
-  if (forced == 32 || forced == 64 || forced == 128) return forced;
   static const int sms = [] { int dev = 0, n = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n; }();
   int block = kBlock;
   while (block > 32 && (range + block - 1) / block < sms * 8) block >>= 1;

@@ -15,14 +15,11 @@
 #include "gemb200_jac.h"
 #include "gemb200_kernels.cuh"
 
-#ifndef GEMB200_MINBLOCKS_JAC
-#define GEMB200_MINBLOCKS_JAC 3  /* fp32: <= 168 registers */
-#endif
-#ifndef GEMB200_MINBLOCKS_JAC_F64
-#define GEMB200_MINBLOCKS_JAC_F64 2  /* fp64: <= 255 registers */
-#endif
-
 namespace gemb200 {
+
+// launch bounds of the three tangent kernels
+constexpr int kMinBlocksJac = 3;  // fp32: <= 168 registers
+constexpr int kMinBlocksJacF64 = 2;  // fp64: <= 255 registers
 
 // radians per unit of the stored angle (turns in the fp32 build, radians in fp64)
 template <typename real> __device__ __forceinline__ real rad_per_ang() { return sizeof(real) == 4 ? real(6.283185307179586) : real(1); }
@@ -738,7 +735,7 @@ __device__ __forceinline__ void jac_loop(const StepParams<real>& p, const JacOut
 // The rollout-Jacobian kernel: rollout_kernel (row-per-env layout, general or ENVP coefficients, no dead time) with jac_loop.  Dynamic shared
 // memory: the observation rows of the block, then its Jacobian rows (jstride words per env).
 template <int FAM, bool FINITE, typename real, int NREF, bool ENVP>
-__global__ void __launch_bounds__(GEMB200_BLOCK, (sizeof(real) == 4 ? GEMB200_MINBLOCKS_JAC : GEMB200_MINBLOCKS_JAC_F64))
+__global__ void __launch_bounds__(kBlock, (sizeof(real) == 4 ? kMinBlocksJac : kMinBlocksJacF64))
 jacobian_kernel(const __grid_constant__ StepParams<real> p, const __grid_constant__ JacOut jo, const int jstride) {
   using F = Fam<FAM>;
   constexpr int NX = F::NX, NH = hot_words(NX, NREF), NC = cold_words(NX, NREF);
@@ -926,7 +923,7 @@ __device__ __forceinline__ RetAcc<real> grad_loop(const StepParams<real>& p, con
 // The return-gradient kernel (continuous converters): jacobian_kernel's shape with grad_loop, and rollout_kernel's returns.  Dynamic shared
 // memory: the observation rows of the block, then per env its stash row and its coefficient row (jstride words).
 template <int FAM, typename real, int NREF, bool ENVP>
-__global__ void __launch_bounds__(GEMB200_BLOCK, (sizeof(real) == 4 ? GEMB200_MINBLOCKS_JAC : GEMB200_MINBLOCKS_JAC_F64))
+__global__ void __launch_bounds__(kBlock, (sizeof(real) == 4 ? kMinBlocksJac : kMinBlocksJacF64))
 return_grad_kernel(const __grid_constant__ StepParams<real> p, const __grid_constant__ GradOut go, const int jstride) {
   using F = Fam<FAM>;
   constexpr int NX = F::NX, NH = hot_words(NX, NREF), NC = cold_words(NX, NREF);
@@ -1044,7 +1041,7 @@ __device__ __forceinline__ void psens_loop(const StepParams<real>& p, const PsOu
 // configuration's (po.raw), into its staging row.  Dynamic shared memory: the observation rows of the block, then per env its row of S and
 // coefficient tangents (jstride words).
 template <int FAM, bool FINITE, typename real, int NREF, bool ENVP>
-__global__ void __launch_bounds__(GEMB200_BLOCK, (sizeof(real) == 4 ? GEMB200_MINBLOCKS_JAC : GEMB200_MINBLOCKS_JAC_F64))
+__global__ void __launch_bounds__(kBlock, (sizeof(real) == 4 ? kMinBlocksJac : kMinBlocksJacF64))
 param_sens_kernel(const __grid_constant__ StepParams<real> p, const __grid_constant__ PsOut po, const int jstride) {
   using F = Fam<FAM>;
   constexpr int NX = F::NX, NX1 = NX + (F::EPS ? 1 : 0), NH = hot_words(NX, NREF), NC = cold_words(NX, NREF), NW = ps_words<FAM>();

@@ -32,7 +32,7 @@ template <int FAM, bool FINITE, typename real, int NREF, typename O>
 static cudaError_t launch_tangent_t(const StepParams<real>& p, const O& o, cudaStream_t st) {
   const int jstride = tangent_stride<FAM, FINITE>(o);
   const int range = p.env_end - p.env_begin;
-  int block = GEMB200_BLOCK;
+  int block = kBlock;
   while (block > 32 && (size_t)block * (size_t)(p.row_stride + jstride) * sizeof(real) > 48 * 1024) block >>= 1;
   const size_t smem = (size_t)block * (size_t)(p.row_stride + jstride) * sizeof(real);
   const int grid = (range + block - 1) / block;

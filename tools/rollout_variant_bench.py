@@ -1,5 +1,6 @@
-"""Time the fused rollout (Cont-CC-PMSM-v0) for several builds of the library (register cap / block size variants of rollout_kernel).
-usage: python tools/rollout_variant_bench.py variants/libgemb200_*.so     (each build in its own subprocess: GEMB200_LIB override)"""
+"""Time the fused rollout (Cont-CC-PMSM-v0) for any set of builds of the library, such as the parent commit and a change, each built
+with gym_electric_motor_b200.build.build(out=...).
+usage: python tools/rollout_variant_bench.py parent/libgemb200.so change/libgemb200.so     (each build in its own subprocess: GEMB200_LIB override)"""
 import json
 import os
 import subprocess

@@ -1,5 +1,5 @@
 """Static SASS instructions per source line of one kernel (needs -lineinfo):  python tools/sass_lines.py <obj> <mangled-substring> [top]
-Offline stand-in for tools/ncu_linemix.py (which needs a GPU capture): shows where the code volume is."""
+Shows where a kernel's code volume is, without a GPU."""
 import collections
 import re
 import subprocess

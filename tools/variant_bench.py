@@ -1,5 +1,6 @@
-"""Time the headline kernel for several builds of the library (block size / register cap variants).
-usage: python tools/variant_bench.py build_variants/libgemb200_b*.so     (each run in a subprocess: GEMB200_LIB override)"""
+"""Time the headline kernel for any set of builds of the library, such as the parent commit and a change, each built with
+gym_electric_motor_b200.build.build(out=...).
+usage: python tools/variant_bench.py parent/libgemb200.so change/libgemb200.so     (each run in a subprocess: GEMB200_LIB override)"""
 import json
 import os
 import subprocess
