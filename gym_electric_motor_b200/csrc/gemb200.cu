@@ -1395,6 +1395,8 @@ int gemb200_step_host(gemb200_handle* h, const void* action, void* obs_out, void
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
   DeviceGuard guard(h->cfg.device);
+  // the host streams are non-blocking: wait for whatever the caller queued before (a reset, step, restore, ... on any stream)
+  CUDA_TRY(cudaDeviceSynchronize());
   int rc = ensure_host_buffers(h);
   if (rc) return rc;
   const size_t n = (size_t)h->cfg.n_envs;
@@ -1403,7 +1405,8 @@ int gemb200_step_host(gemb200_handle* h, const void* action, void* obs_out, void
   // streams: the D2H of chunk c overlaps the H2D + launch of chunk c+1 (PCIe is full duplex).  One API call = one RNG id.
   const bool pipelined = h->cfg.layout == GEMB200_LAYOUT_AOS && n >= (size_t)1 << 16;
   const int nchunk = pipelined ? 4 : 1;  // PCIe D2H bound; 4 keeps the copy count low
-  const size_t per = pipelined ? ((n / nchunk + 255) / 256) * 256 : n;
+  // ceil(n / nchunk) rounded up to whole 256-env blocks: the chunks cover every env (the last one may be shorter)
+  const size_t per = pipelined ? (((n + nchunk - 1) / nchunk + 255) / 256) * 256 : n;
   bool first = true;
   for (int c = 0; c < nchunk; ++c) {
     const size_t b = (size_t)c * per, e = (b + per < n) ? b + per : n;
@@ -1438,6 +1441,7 @@ int gemb200_step_host(gemb200_handle* h, const void* action, void* obs_out, void
 int gemb200_reset_host(gemb200_handle* h, const uint8_t* reset_mask, void* obs_out, void* ref_out) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   DeviceGuard guard(h->cfg.device);
+  CUDA_TRY(cudaDeviceSynchronize());  // as in gemb200_step_host
   int rc = ensure_host_buffers(h);
   if (rc) return rc;
   const size_t n = (size_t)h->cfg.n_envs;

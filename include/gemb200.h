@@ -295,7 +295,9 @@ int gemb200_step(gemb200_handle* h, const void* action, void* obs_out, void* ref
                  uint8_t* terminated_out, void* stream);
 
 /* Same call with HOST buffers (pageable or pinned): H2D of the actions, the launch, D2H of the results and a stream
- * synchronise all happen inside.  This is the drop-in for a host-side caller of env.step. */
+ * synchronise all happen inside.  This is the drop-in for a host-side caller of env.step.  Both *_host calls first wait for
+ * all earlier work on the device (cudaDeviceSynchronize), so they see every call queued before them on any stream.
+ * gemb200_reset_host with a mask leaves the unmasked rows of obs_out / ref_out as the caller had them. */
 int gemb200_step_host(gemb200_handle* h, const void* action, void* obs_out, void* ref_out, void* reward_out,
                       uint8_t* terminated_out);
 int gemb200_reset_host(gemb200_handle* h, const uint8_t* reset_mask, void* obs_out, void* ref_out);
