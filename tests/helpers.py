@@ -1,21 +1,27 @@
-"""Shared test helpers: golden-fixture loading and golden-meta -> gemb200_config translation.
+"""Shared test helpers: golden-fixture loading and golden-meta -> gemb200_config translation, the golden-based device configurations and
+random actions of the parity and rollout tests, the per-env parameter cases, and a handle stand-in for argument checks without a GPU.
 
 The translation here is deliberately independent of the product's own spec compiler
 (gym_electric_motor_b200/spec.py): it takes limits / weights verbatim from the values the REFERENCE reported
 when the golden was recorded, so oracle-vs-golden tests do not depend on the product's host logic.
 """
+import ctypes as C
 import glob
 import json
 import os
 import sys
 
 import numpy as np
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+import torch  # noqa: E402
+
 from gym_electric_motor_b200 import _cabi as K  # noqa: E402
+from gym_electric_motor_b200.vector_sim import VectorSim  # noqa: E402
 
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
@@ -274,3 +280,193 @@ def col_rel_err(a, b):
     a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
     scale = np.maximum(np.abs(b).max(axis=0), 1e-12)
     return float((np.abs(a - b).max(axis=0) / scale).max())
+
+
+# ------------------------------------------------------------------------------------------------- device configurations of the goldens
+TOL = {K.F64: 1e-9, K.F32: 1e-5}
+# dopri5 goldens are compared against RK4 with 2 sub-steps: accuracy of the substitute solver, not identity
+TOL_DOPRI = {K.F64: 2e-6, K.F32: 1e-5}
+# SCIM with dq actions transformed by the FluxObserver's angle: psi_obs is a running sum of current samples with heavy cancellation
+# under random actions, so rounding-level differences of the currents (1e-7 relative in fp32, 1e-16 in fp64) come back amplified
+# ~100x through angle(psi_obs) into the applied voltages.  Conditioning of the configuration, not of the kernel: the same
+# trajectories without that feedback (scim_cc_flux_rk4) hold the plain tolerance.
+TOL_OBSERVER_FEEDBACK = {K.F64: 1e-8, K.F32: 1e-3}
+
+
+def _tol(name, dtype, is_dopri=False, batch=False):
+    if "flux_dq" in name or "flux_cossin_dead1" in name:
+        return TOL_OBSERVER_FEEDBACK[dtype]
+    if name.startswith("dfim_fin") and dtype == K.F32:
+        # tau = 1e-5: the rotor flux stays at ~1 % of nominal for the whole run, so the field-frame (dq) columns carry the fp32
+        # flux noise divided by that small magnitude; the frame-independent columns hold 2e-6
+        return 3e-5
+    return (TOL_DOPRI if is_dopri else TOL)[dtype]
+
+
+class DeviceAdapter:
+    """Gives VectorSim the numpy reset/step/set_reference API that helpers.replay_golden drives."""
+
+    def __init__(self, cfg):
+        from gym_electric_motor_b200.vector_sim import VectorSim
+
+        self.sim = VectorSim(cfg)
+
+    def reset(self, mask=None):
+        obs, ref = self.sim.reset(mask)
+        return obs.double().cpu().numpy(), ref.double().cpu().numpy()
+
+    def step(self, action):
+        obs, ref, rew, term = self.sim.step(np.asarray(action))
+        return obs.double().cpu().numpy(), ref.double().cpu().numpy(), rew.double().cpu().numpy(), term.cpu().numpy()
+
+    def set_reference(self, r):
+        self.sim.set_reference(r)
+
+
+def _random_actions(rng, g, n, steps):
+    a = g["actions"]
+    if a.ndim == 1:
+        hi = int(a.max()) + 1
+        return rng.integers(0, max(hi, 2), size=(steps, n, 1)).astype(np.int32)
+    if a.dtype.kind == "i":
+        hi = a.max(axis=0) + 1
+        return (rng.random((steps, n, a.shape[1])) * hi).astype(np.int32)
+    # smooth-ish random actions so that currents build up and constraints trigger
+    base = rng.uniform(-1, 1, size=(steps, n, a.shape[1]))
+    hold = rng.uniform(-1, 1, size=(1, n, a.shape[1]))
+    lo, hi = a.min(), a.max()
+    out = 0.5 * base + 0.5 * hold
+    if lo >= 0:
+        out = np.abs(out)
+    return out
+
+
+# plain / general instantiations, every motor family, the side state that lives outside the registers (switching states, dead-time
+# ring, RC / AC supply, flux observer, external speed profile position, switched generators)
+ROLLOUT_CASES = ["pmsm_cc_rk4", "pmsm_sc_polyload_rk4", "pmsm_fin_sc_rk4", "pmsm_fin_sc_rk4_interlock", "pmsm_cc_euler3", "synrm_cc_rk4",
+                 "eesm_cc_rk4", "eesm_fin_cc_rk4", "scim_cc_rk4", "scim_fin_cc_interlock_rk4", "dfim_cc_rk4", "permex_cc_rk4", "series_cc_rk4",
+                 "shunt_cc_rk4", "extex_cc_rk4", "permex_fin_sc_rc_interlock_rk4", "pmsm_cc_ac_rk4", "pmsm_cc_extspeed_rk4",
+                 "scim_sc_flux_cossin_dead1_rk4", "eesm_cc_rc_dq_dead1_rk4", "pmsm_cc_cossin_rk4", "dfim_cc_flux_dq_rk4",
+                 "extex_fin_cc_interlock2_rk4", "dfim_fin_sc_interlock2_rk4"]
+
+
+def _mk(name, n, dtype, layout, ref_kind=K.REF_WIENER):
+    g = load_golden(name)
+    init = np.array(g["reset_ode"], dtype=float)
+    n_ode = len(init)
+    init[1:] = [0.7, -0.4, 0.02, 0.03, 0.3][: n_ode - 1] if g["meta"]["motor_class"] in ("SquirrelCageInductionMotor", "DoublyFedInductionMotor") else \
+        [0.9, -0.6, 0.5, 0.3][: n_ode - 1]
+    cfg = config_from_meta(g["meta"], n_envs=n, reset_ode=init, dtype=dtype, solver=None, ref_kind=ref_kind, autoreset=K.AUTORESET_SAME_STEP, seed=77,
+                           layout=layout)
+    for r in range(cfg.n_ref):
+        cfg.ref_margin_lo[r], cfg.ref_margin_hi[r] = -0.7, 0.7
+        cfg.ref_init_lo[r], cfg.ref_init_hi[r] = -0.7, 0.7
+        cfg.ref_len_lo[r], cfg.ref_len_hi[r] = 3, 9  # several sub-episode changes inside one rollout
+    cfg.env_index_offset = 12345
+    if cfg.supply_kind == K.SUPPLY_AC1:
+        cfg.supply_param[2] = 0.0
+    return g, cfg
+
+
+# -------------------------------------------------------------------------------------------------------------- per-env parameter cases
+LP_SLOT = dict(a=K.LP_A, b=K.LP_B, c=K.LP_C, j_load=K.LP_J_LOAD)
+# j_rotor enters only the load words (inv_j, omega_lim, omega_lin): it is a slot of the configurations whose load integrates omega, and
+# cannot matter under a constant-speed load (CC configurations), where it is left out
+_DC_SEP = ("r_a", "r_e", "l_a", "l_e", "l_e_prime")
+_IM = ("r_s", "r_r", "l_m", "l_sigs", "l_sigr")
+MOTOR_SLOTS = dict(PermExDc=("r_a", "l_a", "psi_e"), SeriesDc=_DC_SEP, ShuntDc=_DC_SEP, ExtExDc=_DC_SEP, PMSM=("r_s", "l_d", "l_q", "psi_p"),
+                   SynRM=("r_s", "l_d", "l_q"), EESM=("r_s", "l_d", "l_q", "l_m", "r_e", "l_e"), SCIM=_IM, DFIM=_IM)
+# EESM's k is left out: it only refers the excitation circuit to the stator side and back, so every coefficient of the model
+# (derive_coef: r_E, l_M, l_E and 2 / (3 k) enter as k-free ratios) and therefore every output is the same for any k
+# integrating loads with every polynomial term non-zero (the defaults have c = 0, some a = b = 0), so that a, b and c each matter
+LOADS = dict(PermExDc=dict(a=6.0, b=0.05, c=5e-4, j_load=0.02), SeriesDc=dict(a=0.3, b=0.05, c=2e-4, j_load=1e-4),
+             ShuntDc=dict(a=0.6, b=0.02, c=2e-4, j_load=2e-3), ExtExDc=dict(a=0.6, b=0.02, c=2e-4, j_load=2e-3),
+             PMSM=dict(a=2.0, b=0.05, c=5e-3, j_load=1e-3), SynRM=dict(a=0.3, b=0.01, c=1e-5, j_load=1e-4),
+             EESM=dict(a=100.0, b=1.0, c=5e-3, j_load=0.3), SCIM=dict(a=0.3, b=0.01, c=3e-4, j_load=1e-4),
+             DFIM=dict(a=1.0, b=0.02, c=2e-4, j_load=1e-3))
+# the finite PMSM runs at tau = 1e-5, a tenth of the continuous envs' time: stronger load terms and a load inertia comparable to the rotor's
+FINITE_PMSM_LOAD = dict(a=20.0, b=0.5, c=5e-3, j_load=0.04)
+
+
+def _wrappers(*spec):
+    from gym_electric_motor_b200 import physical_system_wrappers as psw
+
+    out = []
+    for kind, arg in spec:
+        out.append(psw.DeadTimeProcessor(steps=arg) if kind == "DeadTime" else psw.FluxObserver() if kind == "FluxObserver"
+                   else psw.DqToAbcActionProcessor.make(arg))
+    return out
+
+
+def _sc(motor_name, **kw):
+    load = dict(load_parameter=dict(LOADS[motor_name]))
+    load.update(kw.pop("load", {}))
+    return dict(load=load, **kw)
+
+
+# id -> (env id, gem.make kwargs); a function so that every make gets fresh wrapper / initializer objects
+ENV_PARAM_CASES = {
+    "sc-permex": lambda: ("Cont-SC-PermExDc-v0", _sc("PermExDc")),
+    "sc-series": lambda: ("Cont-SC-SeriesDc-v0", _sc("SeriesDc")),
+    "sc-shunt": lambda: ("Cont-SC-ShuntDc-v0", _sc("ShuntDc")),
+    "sc-extex": lambda: ("Cont-SC-ExtExDc-v0", _sc("ExtExDc")),
+    "sc-pmsm": lambda: ("Cont-SC-PMSM-v0", _sc("PMSM")),
+    "sc-synrm": lambda: ("Cont-SC-SynRM-v0", _sc("SynRM")),
+    "sc-eesm": lambda: ("Cont-SC-EESM-v0", _sc("EESM")),
+    "sc-scim": lambda: ("Cont-SC-SCIM-v0", _sc("SCIM")),
+    "sc-dfim": lambda: ("Cont-SC-DFIM-v0", _sc("DFIM")),
+    "cc-dfim": lambda: ("Cont-CC-DFIM-v0", {}),
+    # finite converters: a B6 bridge with interlocking time, and a multi converter (two 4QC) on a two-circuit DC motor
+    "fin-sc-pmsm-interlock": lambda: ("Finite-SC-PMSM-v0", _sc("PMSM", converter=dict(interlocking_time=1e-6),
+                                                                               load=dict(load_parameter=dict(FINITE_PMSM_LOAD)))),
+    "fin-cc-extex": lambda: ("Finite-CC-ExtExDc-v0", {}),
+    # dq actions with the angle advance of a dead time in front (the dq advance adv_k)
+    "cc-pmsm-dq-dead": lambda: ("Cont-CC-PMSM-v0", dict(physical_system_wrappers=_wrappers(("DeadTime", 1), ("DqToAbc", "PMSM")))),
+    # dq actions transformed with the FluxObserver's angle
+    "cc-scim-observer-dq": lambda: ("Cont-CC-SCIM-v0", dict(physical_system_wrappers=_wrappers(("FluxObserver", None), ("DqToAbc", "SCIM")))),
+    # random initial states: the reset observation is derived on the device from the env's own coefficients
+    "sc-pmsm-gaussian-init": lambda: ("Cont-SC-PMSM-v0", _sc("PMSM", motor=dict(motor_initializer=dict(random_init="gaussian", random_params=(None, 0.3))),
+                                                             load=dict(load_initializer=dict(random_init="uniform", interval=[[-50.0, 120.0]])))),
+    "sc-scim-uniform-init": lambda: ("Cont-SC-SCIM-v0", _sc("SCIM", motor=dict(motor_initializer=dict(random_init="uniform")))),
+}
+
+
+def motor_of(env_id):
+    return env_id.split("-")[2]
+
+
+# -------------------------------------------------------------------------------------------------------- argument checks without a GPU
+class _NoLaunch:
+    def __getattr__(self, name):
+        raise AssertionError(f"{name} was called: a bad reference feed must be refused before any launch")
+
+
+class NoLaunchSim(VectorSim):
+    """VectorSim on the CPU device whose library calls fail: every check of a feed runs, no launch does"""
+
+    def __init__(self, cfg, reuse_outputs=True):
+        d = [C.c_int32() for _ in range(4)]
+        K.check(K.load_library().gemb200_query_dims(C.byref(cfg), *[C.byref(x) for x in d]), "gemb200_query_dims")
+        self.n_state, self.n_ode, self.n_act, self.n_ref = [x.value for x in d]
+        self.cfg, self.n, self.finite = cfg, int(cfg.n_envs), bool(cfg.finite)
+        self.soa = cfg.layout == K.LAYOUT_SOA
+        self.dtype = torch.float32 if cfg.dtype == K.F32 else torch.float64
+        self.act_dtype = torch.int32 if self.finite else self.dtype
+        self.device = torch.device("cpu")
+        self._lib, self._h, self._reuse, self._out = _NoLaunch(), None, reuse_outputs, None
+
+
+@pytest.fixture
+def no_launch(monkeypatch):
+    import gym_electric_motor_b200.vector_sim as vs
+
+    monkeypatch.setattr(vs, "VectorSim", NoLaunchSim)
+
+
+def _env(**kw):
+    """six PMSM envs with both references fed by the caller (the N = 6 of the argument-check tests)"""
+    import gym_electric_motor_b200 as gem
+
+    rg = gem.reference_generators.MultipleReferenceGenerator([gem.reference_generators.ExternalReferenceGenerator("i_sd"),
+                                                              gem.reference_generators.ExternalReferenceGenerator("i_sq")])
+    return gem.make("Cont-CC-PMSM-v0", num_envs=6, reference_generator=rg, dtype="float32", **kw)

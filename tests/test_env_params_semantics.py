@@ -14,8 +14,7 @@ import pytest
 
 import gym_electric_motor_b200 as gem
 from gym_electric_motor_b200 import _cabi as K
-
-from test_gpu_env_params_oracle import CASES, LP_SLOT, MOTOR_SLOTS, motor_of
+from helpers import ENV_PARAM_CASES, LP_SLOT, MOTOR_SLOTS, motor_of
 
 PARAM_FIELDS = {"motor_param", "load_param"}
 # limits and nominal values derive from the motor parameters (e.g. the torque limit of a synchronous motor); the random initial state
@@ -33,7 +32,7 @@ def _value(cfg, name):
 
 
 def _make(case, motor_parameter=None, load_parameter=None):
-    env_id, kw = CASES[case]()
+    env_id, kw = ENV_PARAM_CASES[case]()
     if motor_parameter:
         kw["motor"] = dict(kw.get("motor", {}), motor_parameter=motor_parameter)
     if load_parameter:
@@ -43,7 +42,7 @@ def _make(case, motor_parameter=None, load_parameter=None):
     return gem.make(env_id, ode_solver=gem.physical_systems.RK4Solver(), seed=17, **kw)
 
 
-@pytest.mark.parametrize("case", list(CASES))
+@pytest.mark.parametrize("case", list(ENV_PARAM_CASES))
 def test_only_parameters_limits_and_documented_constants_follow_the_physical_parameters(case):
     env = _make(case)
     base = env.build_config()

@@ -21,7 +21,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import MP_SLOT
+from gpu_helpers import torch_cuda  # noqa: F401
+from helpers import ENV_PARAM_CASES, LP_SLOT, MOTOR_SLOTS, MP_SLOT, motor_of
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -31,79 +32,14 @@ TOL = {K.F64: 1e-9, K.F32: 1e-5}
 TOL_OBSERVER_FEEDBACK = {K.F64: 1e-8, K.F32: 1e-3}
 MOVES = 1e-3  # a scaled slot must move some output column by this much (column-relative): 100x the fp32 bar
 GROUP, MIXED, STEPS, OFFSET = 37, 16, 64, 3000  # group sizes deliberately not multiples of 32
-LP_SLOT = dict(a=K.LP_A, b=K.LP_B, c=K.LP_C, j_load=K.LP_J_LOAD)
-# j_rotor enters only the load words (inv_j, omega_lim, omega_lin): it is a slot of the configurations whose load integrates omega, and
-# cannot matter under a constant-speed load (CC configurations), where it is left out
-_DC_SEP = ("r_a", "r_e", "l_a", "l_e", "l_e_prime")
-_IM = ("r_s", "r_r", "l_m", "l_sigs", "l_sigr")
-MOTOR_SLOTS = dict(PermExDc=("r_a", "l_a", "psi_e"), SeriesDc=_DC_SEP, ShuntDc=_DC_SEP, ExtExDc=_DC_SEP, PMSM=("r_s", "l_d", "l_q", "psi_p"),
-                   SynRM=("r_s", "l_d", "l_q"), EESM=("r_s", "l_d", "l_q", "l_m", "r_e", "l_e"), SCIM=_IM, DFIM=_IM)
-# EESM's k is left out: it only refers the excitation circuit to the stator side and back, so every coefficient of the model
-# (derive_coef: r_E, l_M, l_E and 2 / (3 k) enter as k-free ratios) and therefore every output is the same for any k
 # factor of the slot groups: large, but RK4 at the env's tau stays stable (resistances down, everything else up)
 FACTOR = dict(r_a=0.6, r_e=0.6, r_s=0.6, r_r=0.6)
 DEFAULT_FACTOR = 1.7
-# integrating loads with every polynomial term non-zero (the defaults have c = 0, some a = b = 0), so that a, b and c each matter
-LOADS = dict(PermExDc=dict(a=6.0, b=0.05, c=5e-4, j_load=0.02), SeriesDc=dict(a=0.3, b=0.05, c=2e-4, j_load=1e-4),
-             ShuntDc=dict(a=0.6, b=0.02, c=2e-4, j_load=2e-3), ExtExDc=dict(a=0.6, b=0.02, c=2e-4, j_load=2e-3),
-             PMSM=dict(a=2.0, b=0.05, c=5e-3, j_load=1e-3), SynRM=dict(a=0.3, b=0.01, c=1e-5, j_load=1e-4),
-             EESM=dict(a=100.0, b=1.0, c=5e-3, j_load=0.3), SCIM=dict(a=0.3, b=0.01, c=3e-4, j_load=1e-4),
-             DFIM=dict(a=1.0, b=0.02, c=2e-4, j_load=1e-3))
-# the finite PMSM runs at tau = 1e-5, a tenth of the continuous envs' time: stronger load terms and a load inertia comparable to the rotor's
-FINITE_PMSM_LOAD = dict(a=20.0, b=0.5, c=5e-3, j_load=0.04)
-
 
 # initial speed of the integrating loads with a constant initial state, as a fraction of the speed limit: running envs, where the speed
 # dependent load terms b * omega and c * omega^2 matter within the test's few milliseconds; Cont-SC-PMSM starts from standstill instead,
 # in the static-friction band |omega| <= omega_lim where the load torque is omega_lin * omega
 OMEGA0 = {"sc-pmsm": 0.0}
-
-
-def _wrappers(*spec):
-    from gym_electric_motor_b200 import physical_system_wrappers as psw
-
-    out = []
-    for kind, arg in spec:
-        out.append(psw.DeadTimeProcessor(steps=arg) if kind == "DeadTime" else psw.FluxObserver() if kind == "FluxObserver"
-                   else psw.DqToAbcActionProcessor.make(arg))
-    return out
-
-
-def _sc(motor_name, **kw):
-    load = dict(load_parameter=dict(LOADS[motor_name]))
-    load.update(kw.pop("load", {}))
-    return dict(load=load, **kw)
-
-
-# id -> (env id, gem.make kwargs); a function so that every make gets fresh wrapper / initializer objects
-CASES = {
-    "sc-permex": lambda: ("Cont-SC-PermExDc-v0", _sc("PermExDc")),
-    "sc-series": lambda: ("Cont-SC-SeriesDc-v0", _sc("SeriesDc")),
-    "sc-shunt": lambda: ("Cont-SC-ShuntDc-v0", _sc("ShuntDc")),
-    "sc-extex": lambda: ("Cont-SC-ExtExDc-v0", _sc("ExtExDc")),
-    "sc-pmsm": lambda: ("Cont-SC-PMSM-v0", _sc("PMSM")),
-    "sc-synrm": lambda: ("Cont-SC-SynRM-v0", _sc("SynRM")),
-    "sc-eesm": lambda: ("Cont-SC-EESM-v0", _sc("EESM")),
-    "sc-scim": lambda: ("Cont-SC-SCIM-v0", _sc("SCIM")),
-    "sc-dfim": lambda: ("Cont-SC-DFIM-v0", _sc("DFIM")),
-    "cc-dfim": lambda: ("Cont-CC-DFIM-v0", {}),
-    # finite converters: a B6 bridge with interlocking time, and a multi converter (two 4QC) on a two-circuit DC motor
-    "fin-sc-pmsm-interlock": lambda: ("Finite-SC-PMSM-v0", _sc("PMSM", converter=dict(interlocking_time=1e-6),
-                                                                               load=dict(load_parameter=dict(FINITE_PMSM_LOAD)))),
-    "fin-cc-extex": lambda: ("Finite-CC-ExtExDc-v0", {}),
-    # dq actions with the angle advance of a dead time in front (the dq advance adv_k)
-    "cc-pmsm-dq-dead": lambda: ("Cont-CC-PMSM-v0", dict(physical_system_wrappers=_wrappers(("DeadTime", 1), ("DqToAbc", "PMSM")))),
-    # dq actions transformed with the FluxObserver's angle
-    "cc-scim-observer-dq": lambda: ("Cont-CC-SCIM-v0", dict(physical_system_wrappers=_wrappers(("FluxObserver", None), ("DqToAbc", "SCIM")))),
-    # random initial states: the reset observation is derived on the device from the env's own coefficients
-    "sc-pmsm-gaussian-init": lambda: ("Cont-SC-PMSM-v0", _sc("PMSM", motor=dict(motor_initializer=dict(random_init="gaussian", random_params=(None, 0.3))),
-                                                             load=dict(load_initializer=dict(random_init="uniform", interval=[[-50.0, 120.0]])))),
-    "sc-scim-uniform-init": lambda: ("Cont-SC-SCIM-v0", _sc("SCIM", motor=dict(motor_initializer=dict(random_init="uniform")))),
-}
-
-
-def motor_of(env_id):
-    return env_id.split("-")[2]
 
 
 def slots_of(env_id, cfg):
@@ -120,7 +56,7 @@ def make_config(case, n, dtype):
     is constant (with zero currents the torque and rotor-current terms of the reset observation would be zero)"""
     import gym_electric_motor_b200 as gem
 
-    env_id, kw = CASES[case]()
+    env_id, kw = ENV_PARAM_CASES[case]()
     env = gem.make(env_id, num_envs=n, ode_solver=gem.physical_systems.RK4Solver(), autoreset="same_step", seed=17,
                    dtype="float64" if dtype == K.F64 else "float32", env_index_offset=OFFSET, **kw)
     cfg = env.build_config()
@@ -335,17 +271,8 @@ def oracle_matrix(oracle_lib, case, dtype, n=None):
                 mp_rows=mp_rows, lp_rows=lp_rows)
 
 
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-
-    if not torch.cuda.is_available():
-        pytest.fail("GPU test selected but no CUDA device is visible")
-    return torch
-
-
 @pytest.mark.parametrize("dtype", [K.F64, K.F32], ids=["f64", "f32"])
-@pytest.mark.parametrize("case", list(CASES))
+@pytest.mark.parametrize("case", list(ENV_PARAM_CASES))
 def test_per_env_slot_groups_match_per_group_oracles(torch_cuda, oracle_lib, case, dtype):
     from gym_electric_motor_b200.vector_sim import VectorSim
 

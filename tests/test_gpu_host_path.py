@@ -13,9 +13,8 @@ import numpy as np
 import pytest
 
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_param_snapshot import _draws
-from test_gpu_parity import torch_cuda  # noqa: F401
-from test_gpu_rollout import _mk
+from gpu_helpers import _draws, torch_cuda  # noqa: F401
+from helpers import _mk
 
 pytestmark = pytest.mark.gpu
 

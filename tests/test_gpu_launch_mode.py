@@ -1,43 +1,28 @@
-"""Which step / rollout instantiation a handle launches as its per-env parameters, draws, RNG identities and peer destinations come and go.
+"""Which kernel and instantiation a handle launches: the step / rollout instantiation as its per-env parameters, draws, RNG identities and
+peer destinations come and go, and the kernels of a reference feed, of Jacobians, of parameter sensitivities, of return gradients and of
+discounted returns.
 
 The PLAIN, general and ENVP instantiations give bit-identical results (DESIGN.md §2), so no output test notices a handle that takes the
-wrong one; only its speed does (DESIGN.md §4: shared coefficients against per-env blocks).  This test reads the instantiation from the
-kernel name that torch.profiler records: PLAIN is the 6th and ENVP the 8th template argument of step_kernel / rollout_kernel."""
+wrong one; only its speed does (DESIGN.md §4: shared coefficients against per-env blocks).  These tests read the kernel and its
+instantiation from the kernel names that torch.profiler records (gpu_helpers._kernels).  The module runs before the suite's long GPU
+modules: later in a full `-m gpu` session the profiler records no kernels at all."""
 import ctypes as C
-import re
 
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
+from gpu_helpers import _kernels, torch_cuda  # noqa: F401
+from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
 
 N = 4096
-
-
-def _modes(torch, fn):
-    """instantiations ("PLAIN", "ENVP" or "general") of the step and rollout kernels that fn() launches"""
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    modes = []
-    for e in prof.events():
-        m = re.search(r"(step_kernel|rollout_kernel)<([^>]*)>", e.name)
-        if not m:
-            continue
-        args = [a.strip() for a in m.group(2).split(",")]
-        on = [a in ("true", "(bool)1", "1") for a in args]
-        modes.append((m.group(1), "PLAIN" if on[5] else ("ENVP" if on[7] else "general")))
-    return modes
+NAMES = ["r_s", "l_d", "l_q", "psi_p"]
 
 
 def test_launch_mode_transitions(torch_cuda):
     torch = torch_cuda
     import gym_electric_motor_b200 as gem
-    from gym_electric_motor_b200 import _cabi as K
 
     # bench.py's pmsm workload at a small size: fp32, AoS, RK4 (the PLAIN shape)
     env = gem.make("Cont-CC-PMSM-v0", num_envs=N, device="cuda", dtype="float32", ode_solver=gem.physical_systems.RK4Solver(),
@@ -77,12 +62,139 @@ def test_launch_mode_transitions(torch_cuda):
         ("shared parameters, one peer destination", lambda: (env.set_env_parameters(), bind_peers(1)), "general"),
         ("no peer destinations", lambda: bind_peers(0), "PLAIN"),
     ]
-    _modes(torch, lambda: env.step(act()))  # the profiler's first session pays its set-up
+    _kernels(torch, lambda: env.step(act()))  # the profiler's first session pays its set-up
     seen, want = [], []
     for k, (what, change, expected) in enumerate(transitions):
         change()
-        got = _modes(torch, lambda: env.step(act())) + _modes(torch, lambda: env.rollout(act(2), record_every=1))
+        got = _kernels(torch, lambda: env.step(act())) + _kernels(torch, lambda: env.rollout(act(2), record_every=1))
         assert [kernel for kernel, _ in got] == ["step_kernel", "rollout_kernel"], (k, what, got)
         seen.append((k, what, [mode for _, mode in got]))
         want.append((k, what, [expected, expected]))
     assert seen == want
+
+
+def _make(n, dtype="float32", seed=0):
+    """bench.py's pmsm workload: fp32, AoS, RK4 (the PLAIN shape)"""
+    import gym_electric_motor_b200 as gem
+
+    env = gem.make("Cont-CC-PMSM-v0", num_envs=n, device="cuda", dtype=dtype, ode_solver=gem.physical_systems.RK4Solver(), autoreset="same_step",
+                   seed=seed)
+    env.reset()
+    return env
+
+
+def test_feed_launch_modes(torch_cuda):
+    """a step and a rollout with a reference feed: never PLAIN (the PLAIN kernels have no feed), general with shared coefficients, ENVP with
+    per-env parameter blocks; without a feed the PLAIN shape keeps its PLAIN kernels"""
+    torch = torch_cuda
+    env = _make(N)
+    acts = torch.zeros(2, N, 3, device="cuda")
+    refs = torch.zeros(2, N, 2, device="cuda")
+
+    def modes(feed):  # a step and a rollout in one profiler session
+        if feed:
+            return sorted(_kernels(torch, lambda: (env.step(acts[0], reference=refs[0]), env.rollout(acts, record_every=1, references=refs))))
+        return sorted(_kernels(torch, lambda: (env.step(acts[0]), env.rollout(acts, record_every=1))))
+
+    modes(False)  # the profiler's first session pays its set-up
+    assert modes(False) == [("rollout_kernel", "PLAIN"), ("step_kernel", "PLAIN")]
+    assert modes(True) == [("rollout_kernel", "general")] * 2  # step(action, reference=r) is the K = 1 rollout
+    r_s = float(env.sim.cfg.motor_param[K.MP_R_S])
+    env.set_env_parameters(motor_parameter={"r_s": r_s * np.linspace(0.9, 1.1, N)})
+    assert modes(True) == [("rollout_kernel", "ENVP")] * 2
+    env.set_env_parameters()
+    assert modes(False) == [("rollout_kernel", "PLAIN"), ("step_kernel", "PLAIN")]
+
+
+def _tangent_launch_modes(torch, tangent, kernel, identities=True):
+    """a recorded rollout and tangent(env, acts): the tangent kernel, with shared coefficients or (per-env blocks, adopted RNG identities) its
+    ENVP variant, and never a step or rollout kernel; the rollout keeps its PLAIN kernel without per-env state"""
+    env = _make(N)
+    acts = torch.zeros(2, N, 3, device="cuda")
+    both = lambda: (env.rollout(acts, record_every=1), tangent(env, acts))  # noqa: E731
+    _kernels(torch, both)  # the profiler's first session pays its set-up
+    assert sorted(_kernels(torch, both)) == [(kernel, "shared"), ("rollout_kernel", "PLAIN")]
+    r_s = float(env.sim.cfg.motor_param[K.MP_R_S])
+    env.set_env_parameters(motor_parameter={"r_s": r_s * np.linspace(0.9, 1.1, N)})
+    assert sorted(_kernels(torch, both)) == [(kernel, "ENVP"), ("rollout_kernel", "ENVP")]
+    env.set_env_parameters()
+    if identities:
+        env.restore_envs(env.snapshot_envs([0], rng=True), idx=[5], rng="source")
+        assert sorted(_kernels(torch, both)) == [(kernel, "ENVP"), ("rollout_kernel", "ENVP")]
+
+
+def test_jacobian_launch_modes(torch_cuda):
+    _tangent_launch_modes(torch_cuda, lambda env, acts: env.rollout_jacobians(acts), "jacobian_kernel")
+
+
+def test_param_sens_launch_modes(torch_cuda):
+    _tangent_launch_modes(torch_cuda, lambda env, acts: env.rollout_param_sensitivities(acts, NAMES), "param_sens_kernel")
+
+
+@pytest.mark.parametrize("dtype", ["float32", "float64"])
+def test_device_clock_and_cuda_graph(torch_cuda, dtype):
+    """under the device clock rollout_param_sens_into is stream-ordered and capturable: an eager launch and replays of a captured one give,
+    round after round, the bits of host-clock launches on a twin (sens_io refilled with zeros in place before each replay)"""
+    torch = torch_cuda
+    n, k = 1000, 12
+    host, dev, cap = _make(n, dtype), _make(n, dtype), _make(n, dtype)
+    dev.sim.set_device_clock(True)
+    cap.sim.set_device_clock(True)
+    sim = cap.sim
+    slots = cap.param_slots(NAMES)
+    nx = sim.n_ode
+    rng = np.random.default_rng(0)
+    static = torch.zeros(k, n, 3, dtype=sim.dtype, device="cuda")
+    sio = torch.zeros(n, nx, len(NAMES), dtype=sim.dtype, device="cuda")
+    so = torch.empty(k, n, nx, len(NAMES), dtype=sim.dtype, device="cuda")
+    obs = torch.empty((k,) + sim._shape(sim.n_state), dtype=sim.dtype, device="cuda")
+    ref = torch.empty((k,) + sim._shape(sim.n_ref), dtype=sim.dtype, device="cuda")
+    rew = torch.empty(k, n, dtype=sim.dtype, device="cuda")
+    term = torch.empty(k, n, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        sim.rollout_param_sens_into(static, k, slots, sio, so, obs, ref, rew, term)
+    terminated = 0
+    for rnd in range(3):
+        acts = torch.as_tensor(rng.uniform(-1, 1, size=(k, n, 3)), dtype=sim.dtype, device="cuda").contiguous()
+        static.copy_(acts)
+        sio.zero_()
+        graph.replay()
+        (s_h, l_h), ((o_h, r_h), w_h, t_h) = host.rollout_param_sensitivities(acts, NAMES)
+        (s_d, l_d), ((o_d, r_d), w_d, t_d) = dev.rollout_param_sensitivities(acts, NAMES)
+        for name, a, b, c in (("sens", s_h, s_d, so), ("sens_last", l_h, l_d, sio), ("obs", o_h, o_d, obs), ("reward", w_h, w_d, rew)):
+            assert torch.equal(a, b) and torch.equal(a, c), (rnd, name)
+        assert torch.equal(t_h.to(torch.uint8), term)
+        terminated += int(t_h.sum())
+    assert terminated > 0
+    assert host.sim.clock() == dev.sim.clock() == cap.sim.clock()
+
+
+def test_return_grad_launch_modes(torch_cuda):
+    _tangent_launch_modes(torch_cuda, lambda env, acts: env.rollout_return_grads(acts, 0.9), "return_grad_kernel", identities=False)
+
+
+def test_returns_launch_modes(torch_cuda):
+    """a rollout with discounted returns: never PLAIN (the PLAIN kernels have no returns), general with shared coefficients, ENVP with
+    per-env blocks or adopted RNG identities; launches without returns keep their PLAIN kernels"""
+    torch = torch_cuda
+    env = _make(N)
+    acts = torch.zeros(2, N, 3, device="cuda")
+
+    def modes(returns):  # a step, a rollout and (with returns) a scored rollout in one profiler session
+        if returns:
+            return sorted(_kernels(torch, lambda: (env.step(acts[0]), env.rollout(acts, record_every=0), env.rollout_returns(acts, 0.9))))
+        return sorted(_kernels(torch, lambda: (env.step(acts[0]), env.rollout(acts, record_every=0))))
+
+    modes(False)  # the profiler's first session pays its set-up
+    plain = [("rollout_kernel", "PLAIN"), ("step_kernel", "PLAIN")]
+    assert modes(False) == plain
+    assert modes(True) == [("rollout_kernel", "PLAIN"), ("rollout_kernel", "general"), ("step_kernel", "PLAIN")]
+    r_s = float(env.sim.cfg.motor_param[K.MP_R_S])
+    env.set_env_parameters(motor_parameter={"r_s": r_s * np.linspace(0.9, 1.1, N)})
+    assert modes(True) == [("rollout_kernel", "ENVP")] * 2 + [("step_kernel", "ENVP")]
+    env.set_env_parameters()
+    assert modes(False) == plain
+    env.restore_envs(env.snapshot_envs([0], rng=True), idx=[5], rng="source")  # adopted identities: the ENVP kernels read them
+    assert modes(True) == [("rollout_kernel", "ENVP")] * 2 + [("step_kernel", "ENVP")]

@@ -18,7 +18,7 @@ import pytest
 
 from helpers import load_golden, config_from_meta, switched_config
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import torch_cuda  # noqa: F401  (fixture)
+from gpu_helpers import torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import torch_cuda  # noqa: F401
+from gpu_helpers import torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

@@ -11,8 +11,8 @@ check does not rest on the device's own primal step.  Per case:
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
-from test_gpu_param_sensitivities import SLOT, _wrap
+from fd_helpers import SLOT, _oracle_states, _wrap, build_up_flux, sens_check
+from gpu_helpers import torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -47,20 +47,6 @@ def _config(env_id, m, load):
     return cfg
 
 
-def _oracle_states(cfg, x0, acts):
-    """the oracle's ODE state after every step from x0: [K, m, n_x]"""
-    from oracle.gem_oracle import Oracle
-
-    o = Oracle(cfg)
-    o.reset()
-    o.set_ode_state(x0)
-    xs = []
-    for a in acts:
-        o.step(a)
-        xs.append(o.get_ode_state())
-    return np.stack(xs)
-
-
 @pytest.mark.parametrize("load", ["poly", "const"])
 @pytest.mark.parametrize("motor", list(MOTORS))
 def test_against_central_differences_of_the_oracle(torch_cuda, motor, load):
@@ -77,9 +63,7 @@ def test_against_central_differences_of_the_oracle(torch_cuda, motor, load):
     x0 = sim.get_ode_state().cpu().numpy()
     x0[:, 0] = np.linspace(-150, 150, m)  # running speeds of both signs, outside the static-friction band
     has_eps = cfg.motor_kind >= K.MOTOR_PMSM
-    if cfg.motor_kind in (K.MOTOR_SCIM, K.MOTOR_DFIM):  # a built-up rotor flux
-        mag, ang = rng.uniform(0.2, 0.8, m), rng.uniform(-np.pi, np.pi, m)
-        x0[:, 3], x0[:, 4] = mag * np.cos(ang), mag * np.sin(ang)
+    build_up_flux(rng, cfg, x0)
     if has_eps:
         x0[:, -1] = rng.uniform(-2.5, 2.5, m)
     sim.set_ode_state(x0)
@@ -110,16 +94,11 @@ def test_against_central_differences_of_the_oracle(torch_cuda, motor, load):
         dup, ddn = side[0] - mid, mid - side[1]
         if has_eps:
             dup[..., -1], ddn[..., -1] = _wrap(dup[..., -1]), _wrap(ddn[..., -1])
-        fd = (dup + ddn) / (2 * h)  # [K, m, n_x]
+        fd, scale, err, kink, bad = sens_check(s[..., j], dup, ddn, mid, h, TOL)  # [K, m, n_x]
         if load == "const" and nm in MECH:
             assert np.all(s[..., j] == 0) and np.all(fd == 0), (motor, nm, "a parameter that does not enter: exact 0")
             continue
-        floor = 64 * 2.2e-16 * (np.abs(mid) + 1) / h
-        scale = np.abs(fd).max(axis=2, keepdims=True)
         assert scale.max() > 0, (motor, nm, "the parameter moves the trajectory")
-        kink = (np.abs(dup - ddn) / h > 1e-2 * scale + floor).any(axis=2)
-        err = np.abs(s[..., j] - fd)
-        bad = (err > TOL * scale + floor).any(axis=2) & ~kink
         kinks += int(kink.sum())
         total += kink.size
         worst = (err / np.maximum(scale, 1e-300)).max(axis=2)

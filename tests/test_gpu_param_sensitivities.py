@@ -11,11 +11,9 @@ S = d x / d theta of every env's own physical parameters.
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
-from test_gpu_rollout_jacobians import _cfg
-from test_gpu_rollout_returns import ENV_IDS, _actions, _blob, _eq, _make, _next_steps, _same
+from fd_helpers import SLOT, _cfg, _wrap, build_up_flux, currents_off_zero, sens_check, switching_states
+from gpu_helpers import ENV_IDS, _actions, _blob, _eq, _make, _next_steps, _same, torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
-from gym_electric_motor_b200.core import ElectricMotorEnvironment
 
 pytestmark = pytest.mark.gpu
 
@@ -128,15 +126,6 @@ def test_carry_against_the_jacobian_recursion(torch_cuda, family):
         assert err <= 1e-12, (family, j, err)
 
 
-def _wrap(d):
-    return (d + np.pi) % (2 * np.pi) - np.pi
-
-
-SLOT = {**{nm: s for nm, s in ElectricMotorEnvironment._MP_SLOT.items()},
-        **{nm: K.MAX_MOTOR_PARAM + s for nm, s in ElectricMotorEnvironment._LP_SLOT.items()}}
-_N_SWITCH = {K.CONV_B6: 8, K.CONV_4QC: 4, K.CONV_2QC: 3, K.CONV_1QC: 2, K.CONV_NONE: 1}
-
-
 def _fd_case(torch, env_id, names, k, m=16, dtype="float64", rel_h=1e-4, tol=1e-7, omega=None, expect_zero=(), tweak=None, **cfg_kw):
     """central differences of the float64 step against S of a `dtype` handle: the perturbed copies theta_j (1 +- h) are envs of ONE float64
     handle with per-env blocks, driven one step per launch so that every step's state can be read.  Every entry must be within tol of its
@@ -168,17 +157,12 @@ def _fd_case(torch, env_id, names, k, m=16, dtype="float64", rel_h=1e-4, tol=1e-
     if omega is not None:
         x0[:, 0] = omega
     has_eps = c_s.motor_kind >= K.MOTOR_PMSM
-    if c_s.motor_kind in (K.MOTOR_SCIM, K.MOTOR_DFIM):  # a built-up rotor flux
-        mag, ang = rng.uniform(0.2, 0.8, m), rng.uniform(-np.pi, np.pi, m)
-        x0[:, 3], x0[:, 4] = mag * np.cos(ang), mag * np.sin(ang)
-    if ss.finite:  # no current at 0: there a leg in its interlock state switches its voltage with the current's sign
-        cur = slice(1, 3 if has_eps else x0.shape[1])
-        x0[:, cur] += rng.choice([-1.0, 1.0], x0[:, cur].shape) * rng.uniform(0.5, 2.0, x0[:, cur].shape)
+    build_up_flux(rng, c_s, x0)
+    currents_off_zero(rng, c_s, x0)
     ss.set_ode_state(x0)
     fd.set_ode_state(np.tile(x0, (copies, 1)))
     if ss.finite:
-        hi = np.array([_N_SWITCH[c_s.converter_kind[j]] for j in range(ss.n_act)])
-        a = rng.integers(0, hi, (k, m, ss.n_act))
+        a = switching_states(rng, c_s, (k, m, ss.n_act))
         acts = torch.as_tensor(a, dtype=torch.int32, device="cuda").contiguous()
     else:
         a = rng.uniform(-0.9, 0.9, (k, m, ss.n_act))
@@ -198,18 +182,12 @@ def _fd_case(torch, env_id, names, k, m=16, dtype="float64", rel_h=1e-4, tol=1e-
             if has_eps:
                 for v in (dup, ddn, dup2, ddn2):
                     v[:, -1] = _wrap(v[:, -1])
-            d = (dup + ddn) / (2 * h[j])
             # the reference's own error: each row's rounding floor, and twice the distance to the 2h difference (that distance is 3/4 of
             # the 2h difference's truncation error, i.e. 3x the h difference's, plus rounding that reaches the row from the other states)
-            rnd = 64 * 2.2e-16 * (np.abs(mid) + 1) / h[j]
-            floor = rnd + 2 * np.abs(d - (dup2 + ddn2) / (4 * h[j]))
-            scale = np.abs(d).max(axis=1, keepdims=True)
+            d, scale, err, kink, bad = sens_check(s[:, :, j], dup, ddn, mid, h[j], tol, d2h=(dup2 + ddn2) / (4 * h[j]))
             if names[j] in expect_zero:
                 assert np.all(s[:, :, j] == 0) and np.all(d == 0), (env_id, names[j], "a parameter that does not enter: exact 0")
                 continue
-            kink = (np.abs(dup - ddn) / h[j] > 1e-2 * scale + rnd).any(axis=1)
-            err = np.abs(s[:, :, j] - d)
-            bad = (err > tol * scale + floor).any(axis=1) & ~kink
             kinks += int(kink.sum())
             total += m
             assert not bad.any(), (env_id, dtype, names[j], step, (err / np.maximum(scale, 1e-300)).max(axis=1)[bad].max())

@@ -7,26 +7,12 @@ import numpy as np
 import pytest
 
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import torch_cuda  # noqa: F401
-from test_gpu_rng_identity import SCIM_RANDOM, _acts, _cfg, _run, _same
-from test_gpu_rollout import _dev_actions
+from gpu_helpers import _MOTOR_SLOTS, SCIM_RANDOM, _acts, _dev_actions, _draws, _random_cfg, _run, _same_outputs, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 CASES_P = ["pmsm_cc_rk4", "eesm_cc_rk4", "permex_cc_rk4", "scim_cc_rk4", SCIM_RANDOM, "dfim_cc_rk4"]
 CROSS_RESETS = ("pmsm_cc_rk4", "eesm_cc_rk4", "permex_cc_rk4")
-_MOTOR_SLOTS = {  # parameters drawn per reset, +-20 % around the configuration's value (induction motors: no flux-limit slots with random init)
-    K.MOTOR_PMSM: (K.MP_R_S, K.MP_L_D, K.MP_L_Q, K.MP_PSI_P, K.MP_J_ROTOR),
-    K.MOTOR_EESM: (K.MP_R_S, K.MP_L_D, K.MP_L_Q, K.MP_R_E, K.MP_J_ROTOR),
-    K.MOTOR_PERMEX_DC: (K.MP_R_A, K.MP_L_A, K.MP_PSI_E, K.MP_J_ROTOR),
-    K.MOTOR_SCIM: (K.MP_J_ROTOR,),
-    K.MOTOR_DFIM: (K.MP_R_S, K.MP_L_M, K.MP_J_ROTOR),
-}
-
-
-def _draws(cfg):
-    slots = [s for s in _MOTOR_SLOTS[cfg.motor_kind] if cfg.motor_param[s] > 0]
-    return (slots, [K.DIST_UNIFORM] * len(slots), [0.8 * cfg.motor_param[s] for s in slots], [1.2 * cfg.motor_param[s] for s in slots])
 
 
 def _config_row(cfg):
@@ -43,8 +29,8 @@ def _randomised_pair(torch, name, dtype, m=120, n_a=301, n_b=403):
     histories; A's envs src are then deep-copied into B's envs dst (state, RNG identity and parameters)"""
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg_a = _cfg(name, n_a, dtype)
-    _, cfg_b = _cfg(name, n_b, dtype, seed=5, offset=999)
+    g, cfg_a = _random_cfg(name, n_a, dtype)
+    _, cfg_b = _random_cfg(name, n_b, dtype, seed=5, offset=999)
     a, b = VectorSim(cfg_a), VectorSim(cfg_b)
     for s in (a, b):
         s.set_param_randomization(*_draws(s.cfg))
@@ -87,7 +73,7 @@ def test_deep_copy_under_draws_replays_the_source(torch_cuda, name, dtype, mode)
     else:
         out_a, out_b = _run(torch, a, da, mode, si), _run(torch, b, db, mode, di)
         _same_params(torch, a, b, src, dst, mode)
-    _same(torch, out_a, out_b, (name, mode))
+    _same_outputs(torch, out_a, out_b, (name, mode))
     if name in CROSS_RESETS:
         assert sum(int(o[3].sum().item()) for o in out_a) > 0, "the case is meant to cross terminations + in-kernel resets after the restore"
     ra, rb = a.reset(), b.reset()  # an explicit reset draws the source's values as well
@@ -104,8 +90,8 @@ def test_own_identity_with_source_parameters_draws_its_own_at_the_next_reset(tor
     from gym_electric_motor_b200.vector_sim import VectorSim
 
     name = "pmsm_cc_rk4"
-    g, cfg_a = _cfg(name, 301, dtype)
-    _, cfg_b = _cfg(name, 403, dtype, seed=5, offset=999)
+    g, cfg_a = _random_cfg(name, 301, dtype)
+    _, cfg_b = _random_cfg(name, 403, dtype, seed=5, offset=999)
     a, b, twin = VectorSim(cfg_a), VectorSim(cfg_b), VectorSim(cfg_b)
     for s in (a, b, twin):
         s.set_param_randomization(*_draws(s.cfg))
@@ -124,7 +110,7 @@ def test_own_identity_with_source_parameters_draws_its_own_at_the_next_reset(tor
     assert torch.equal(b.env_params(), twin.env_params())
     everyone = torch.arange(b.n, device=b.device)
     da = _dev_actions(torch, b, _acts(rng, g, b, 12))
-    _same(torch, _run(torch, b, da, "step", everyone), _run(torch, twin, da, "step", everyone), "after the reset")
+    _same_outputs(torch, _run(torch, b, da, "step", everyone), _run(torch, twin, da, "step", everyone), "after the reset")
     for s in (a, b, twin):
         s.close()
 
@@ -144,8 +130,8 @@ def test_host_set_blocks_restored_into_shared_coefficients(torch_cuda, name, dty
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg_a = _cfg(name, 301, dtype)
-    _, cfg_b = _cfg(name, 403, dtype, seed=5, offset=999)
+    g, cfg_a = _random_cfg(name, 301, dtype)
+    _, cfg_b = _random_cfg(name, 403, dtype, seed=5, offset=999)
     a, b, twin = VectorSim(cfg_a), VectorSim(cfg_b), VectorSim(cfg_b)
     rng = np.random.default_rng(5)
     mp = np.tile(np.array(list(cfg_a.motor_param)), (a.n, 1))
@@ -169,7 +155,7 @@ def test_host_set_blocks_restored_into_shared_coefficients(torch_cuda, name, dty
     out_b = _run(torch, b, db, "step", everyone)
     out_t = _run(torch, twin, db, "step", everyone)
     di = torch.as_tensor(dst, device=b.device)
-    _same(torch, out_a, [tuple(t[di] for t in o) for o in out_b], "the restored envs replay their sources")
+    _same_outputs(torch, out_a, [tuple(t[di] for t in o) for o in out_b], "the restored envs replay their sources")
     keep = torch.ones(b.n, dtype=torch.bool, device=b.device)
     keep[di] = False
     induction = name.startswith(("scim", "dfim"))
@@ -190,8 +176,8 @@ def test_mpc_step_on_randomised_plants_matches_its_best_branch(torch_cuda):
     from gym_electric_motor_b200.vector_sim import VectorSim
 
     plants, cand, horizon = 16, 32, 6
-    g, cfg_p = _cfg("pmsm_cc_rk4", plants, K.F32)
-    _, cfg_m = _cfg("pmsm_cc_rk4", plants * cand, K.F32, seed=8, offset=0)
+    g, cfg_p = _random_cfg("pmsm_cc_rk4", plants, K.F32)
+    _, cfg_m = _random_cfg("pmsm_cc_rk4", plants * cand, K.F32, seed=8, offset=0)
     p, mdl = VectorSim(cfg_p), VectorSim(cfg_m)
     for s in (p, mdl):
         s.set_param_randomization(*_draws(s.cfg))
@@ -220,8 +206,8 @@ def test_edited_parameters_equal_host_set_rows(torch_cuda, dtype):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg_a = _cfg("pmsm_cc_rk4", 301, dtype)
-    _, cfg_b = _cfg("pmsm_cc_rk4", 403, dtype, seed=5, offset=999)
+    g, cfg_a = _random_cfg("pmsm_cc_rk4", 301, dtype)
+    _, cfg_b = _random_cfg("pmsm_cc_rk4", 403, dtype, seed=5, offset=999)
     a, c, b = VectorSim(cfg_a), VectorSim(cfg_a), VectorSim(cfg_b)
     for s in (a, b, c):
         s.reset()
@@ -244,7 +230,7 @@ def test_edited_parameters_equal_host_set_rows(torch_cuda, dtype):
     db[:, dst] = da[:, src]
     out_c = _run(torch, c, _dev_actions(torch, c, da), "step", torch.as_tensor(src, device=c.device))
     out_b = _run(torch, b, _dev_actions(torch, b, db), "step", torch.as_tensor(dst, device=b.device))
-    _same(torch, out_c, out_b, "edited r_s")
+    _same_outputs(torch, out_c, out_b, "edited r_s")
     for s in (a, b, c):
         s.close()
 
@@ -254,7 +240,7 @@ def test_pack_without_blocks_and_round_trip(torch_cuda):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg = _cfg("eesm_cc_rk4", 257, K.F64)
+    g, cfg = _random_cfg("eesm_cc_rk4", 257, K.F64)
     h, twin = VectorSim(cfg), VectorSim(cfg)
     snap = h.snapshot(params=True)
     assert snap.pole_pairs == cfg.motor_param[K.MP_P]
@@ -270,7 +256,7 @@ def test_pack_without_blocks_and_round_trip(torch_cuda):
     h.restore(h.snapshot(params=True), params="source")  # every env into itself
     assert torch.equal(h.env_params(), twin.env_params())
     everyone = torch.arange(h.n, device=h.device)
-    _same(torch, _run(torch, h, acts[10:], "step", everyone), _run(torch, twin, acts[10:], "step", everyone), "round trip")
+    _same_outputs(torch, _run(torch, h, acts[10:], "step", everyone), _run(torch, twin, acts[10:], "step", everyone), "round trip")
     assert torch.equal(h.env_params(), twin.env_params())
     h.close()
     twin.close()
@@ -281,7 +267,7 @@ def test_captured_pack_and_unpack_give_the_eager_bits(torch_cuda):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg = _cfg("pmsm_cc_rk4", 300, K.F32)
+    g, cfg = _random_cfg("pmsm_cc_rk4", 300, K.F32)
     eager, cap = VectorSim(cfg), VectorSim(cfg)
     rng = np.random.default_rng(9)
     acts = _dev_actions(torch, eager, _acts(rng, g, eager, 30))
@@ -304,7 +290,7 @@ def test_captured_pack_and_unpack_give_the_eager_bits(torch_cuda):
     torch.cuda.synchronize()
     assert torch.equal(eager.env_params(), cap.env_params())
     everyone = torch.arange(cap.n, device=cap.device)
-    _same(torch, _run(torch, eager, acts[8:], "step", everyone), _run(torch, cap, acts[8:], "step", everyone), "captured pack / unpack")
+    _same_outputs(torch, _run(torch, eager, acts[8:], "step", everyone), _run(torch, cap, acts[8:], "step", everyone), "captured pack / unpack")
     assert torch.equal(eager.env_params(), cap.env_params())
     eager.close()
     cap.close()
@@ -315,7 +301,7 @@ def test_paths_without_params_stay_refused_under_draws(torch_cuda):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    _, cfg = _cfg("pmsm_cc_rk4", 64, K.F32)
+    _, cfg = _random_cfg("pmsm_cc_rk4", 64, K.F32)
     d = VectorSim(cfg)
     d.set_param_randomization(*_draws(d.cfg))
     d.reset()

@@ -8,59 +8,12 @@ column-relative — the bar BASELINE.json's north_star sets for state trajectori
 import numpy as np
 import pytest
 
-from helpers import golden_reset_state, switched_config, col_rel_err, config_from_meta, golden_names, load_golden, replay_golden
+from gpu_helpers import torch_cuda  # noqa: F401
+from helpers import (TOL, DeviceAdapter, _random_actions, _tol, col_rel_err, config_from_meta, golden_names, golden_reset_state,
+                     load_golden, replay_golden, switched_config)
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
-
-TOL = {K.F64: 1e-9, K.F32: 1e-5}
-# dopri5 goldens are compared against RK4 with 2 sub-steps: accuracy of the substitute solver, not identity
-TOL_DOPRI = {K.F64: 2e-6, K.F32: 1e-5}
-# SCIM with dq actions transformed by the FluxObserver's angle: psi_obs is a running sum of current samples with heavy cancellation
-# under random actions, so rounding-level differences of the currents (1e-7 relative in fp32, 1e-16 in fp64) come back amplified
-# ~100x through angle(psi_obs) into the applied voltages.  Conditioning of the configuration, not of the kernel: the same
-# trajectories without that feedback (scim_cc_flux_rk4) hold the plain tolerance.
-TOL_OBSERVER_FEEDBACK = {K.F64: 1e-8, K.F32: 1e-3}
-
-
-def _tol(name, dtype, is_dopri=False, batch=False):
-    if "flux_dq" in name or "flux_cossin_dead1" in name:
-        return TOL_OBSERVER_FEEDBACK[dtype]
-    if name.startswith("dfim_fin") and dtype == K.F32:
-        # tau = 1e-5: the rotor flux stays at ~1 % of nominal for the whole run, so the field-frame (dq) columns carry the fp32
-        # flux noise divided by that small magnitude; the frame-independent columns hold 2e-6
-        return 3e-5
-    return (TOL_DOPRI if is_dopri else TOL)[dtype]
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-
-    if not torch.cuda.is_available():
-        pytest.fail("GPU test selected but no CUDA device is visible")
-    return torch
-
-
-class DeviceAdapter:
-    """Gives VectorSim the numpy reset/step/set_reference API that helpers.replay_golden drives."""
-
-    def __init__(self, cfg):
-        from gym_electric_motor_b200.vector_sim import VectorSim
-
-        self.sim = VectorSim(cfg)
-
-    def reset(self, mask=None):
-        obs, ref = self.sim.reset(mask)
-        return obs.double().cpu().numpy(), ref.double().cpu().numpy()
-
-    def step(self, action):
-        obs, ref, rew, term = self.sim.step(np.asarray(action))
-        return obs.double().cpu().numpy(), ref.double().cpu().numpy(), rew.double().cpu().numpy(), term.cpu().numpy()
-
-    def set_reference(self, r):
-        self.sim.set_reference(r)
-
 
 def _golden_cases():
     out = []
@@ -123,24 +76,6 @@ BATCH_CASES = [
     # state-vector wrappers (CosSinProcessor, FluxObserver, FluxObserver angle for dq actions, dead time in front)
     ("pmsm_cc_cossin_rk4", "rk4"), ("pmsm_sc_cossin_rm_rk4", "rk4"), ("scim_cc_flux_dq_rk4", "rk4"), ("scim_sc_flux_cossin_dead1_rk4", "rk4"),
 ]
-
-
-def _random_actions(rng, g, n, steps):
-    a = g["actions"]
-    if a.ndim == 1:
-        hi = int(a.max()) + 1
-        return rng.integers(0, max(hi, 2), size=(steps, n, 1)).astype(np.int32)
-    if a.dtype.kind == "i":
-        hi = a.max(axis=0) + 1
-        return (rng.random((steps, n, a.shape[1])) * hi).astype(np.int32)
-    # smooth-ish random actions so that currents build up and constraints trigger
-    base = rng.uniform(-1, 1, size=(steps, n, a.shape[1]))
-    hold = rng.uniform(-1, 1, size=(1, n, a.shape[1]))
-    lo, hi = a.min(), a.max()
-    out = 0.5 * base + 0.5 * hold
-    if lo >= 0:
-        out = np.abs(out)
-    return out
 
 
 @pytest.mark.parametrize("dtype", [K.F64, K.F32], ids=["f64", "f32"])

@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 
 from helpers import col_rel_err, config_from_meta, golden_names, load_golden, replay_golden
-from test_gpu_parity import DeviceAdapter, _tol, torch_cuda  # noqa: F401
+from gpu_helpers import torch_cuda  # noqa: F401
+from helpers import DeviceAdapter, _tol
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu

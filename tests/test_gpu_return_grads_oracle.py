@@ -13,7 +13,8 @@ A CPU test (test_return_grads_oracle_harness.py) checks the harness itself again
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
+from fd_helpers import build_up_flux, clip_angle, compare_fd, oracle_fd
+from gpu_helpers import torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -33,99 +34,6 @@ _KEEP = []
 # ------------------------------------------------------------------------------------------------------------------ the oracle side
 def ode_has_angle(cfg):
     return cfg.motor_kind >= K.MOTOR_PMSM
-
-
-def discount_power(gamma, k):
-    w = 1.0
-    for _ in range(k):
-        w *= gamma
-    return w
-
-
-def oracle_run(make_oracles, warm, x0, ref0, acts, gamma):
-    """the float64 oracle from reset through the warm-up actions, then from (x0, ref0) through acts [K, m, nu]: (returns, end steps, x_K).
-    make_oracles() -> [(Oracle, slice of the m envs)]; returns sum gamma^k r_k up to and including the first termination (end = K: none)."""
-    oras = make_oracles()
-    for o, _ in oras:
-        o.reset()
-    for a in warm:
-        for o, sl in oras:
-            o.step(a[sl])
-    for o, sl in oras:
-        o.set_ode_state(x0[sl])
-        if o.n_ref:
-            o.set_reference(ref0[sl])
-    k_steps, m = acts.shape[0], acts.shape[1]
-    ret, end, w = np.zeros(m), np.full(m, k_steps), 1.0
-    for k in range(k_steps):
-        rew, term = np.zeros(m), np.zeros(m, dtype=bool)
-        for o, sl in oras:
-            _, _, rew[sl], t = o.step(acts[k][sl])
-            term[sl] = t.astype(bool)
-        alive = end == k_steps
-        ret[alive] = ret[alive] + w * rew[alive]
-        end[alive & term] = k
-        w = w * gamma
-    return ret, end, np.concatenate([o.get_ode_state() for o, _ in oras])
-
-
-def oracle_fd(make_oracles, warm, x0, acts, gamma, ref0=None, value_grad=None, angle=False):
-    """central differences of the oracle's returns over every column of (x0, a_0 .. a_K-1): one oracle instance set per stencil point.
-    With value_grad [m, n_x], the target is returns + gamma^K value_grad . x_K for the envs with end == K (the angle of x_K unwrapped
-    relative to the unperturbed run).  Returns dict(ret, end, xk, plus, minus, end_p, end_m, h) with [m, n_col] stencil arrays."""
-    m, nx = x0.shape
-    k_steps, _, nu = acts.shape
-    ref0 = np.zeros((m, 0)) if ref0 is None else ref0
-    gk = discount_power(gamma, k_steps)
-    base = oracle_run(make_oracles, warm, x0, ref0, acts, gamma)
-
-    def target(res):
-        ret, end, xk = res
-        if value_grad is None:
-            return ret
-        xk = xk.copy()
-        if angle:
-            d = xk[:, -1] - base[2][:, -1]
-            xk[:, -1] = base[2][:, -1] + (d + np.pi) % (2 * np.pi) - np.pi
-        return np.where(end == k_steps, ret + gk * (value_grad * xk).sum(1), ret)
-
-    ncol = nx + k_steps * nu
-    plus, minus = np.zeros((m, ncol)), np.zeros((m, ncol))
-    end_p, end_m = np.zeros((m, ncol), dtype=int), np.zeros((m, ncol), dtype=int)
-    h = np.zeros(ncol)
-    for c in range(ncol):
-        for sign, val, ends in ((1.0, plus, end_p), (-1.0, minus, end_m)):
-            xs, a = x0.copy(), acts.copy()
-            if c < nx:
-                h[c] = 1e-6 * max(1.0, float(np.abs(x0[:, c]).max()))
-                xs[:, c] += sign * h[c]
-            else:
-                h[c] = 1e-6
-                kk, u = divmod(c - nx, nu)
-                a[kk, :, u] += sign * h[c]
-            res = oracle_run(make_oracles, warm, xs, ref0, a, gamma)
-            val[:, c] = target(res)
-            ends[:, c] = res[1]
-    return dict(ret=base[0], end=base[1], xk=base[2], target=target(base), plus=plus, minus=minus, end_p=end_p, end_m=end_m, h=h)
-
-
-def compare_fd(name, grad, fd, tol):
-    """worst |grad - central difference| relative to each env's gradient scale, over the stencils that stay on one branch: a stencil is
-    excluded when its end steps differ from the unperturbed run's or its one-sided differences disagree by more than 1e-4 of the scale
-    (a termination, a clip, |e|^p at e = 0 on one side).  Returns (worst, excluded, total)."""
-    m, ncol = grad.shape
-    worst, excluded = 0.0, 0
-    for b in range(m):
-        scale = max(np.abs(grad[b]).max(), 1e-12)
-        for c in range(ncol):
-            hc = fd["h"][c]
-            right, left = (fd["plus"][b, c] - fd["target"][b]) / hc, (fd["target"][b] - fd["minus"][b, c]) / hc
-            if fd["end_p"][b, c] != fd["end"][b] or fd["end_m"][b, c] != fd["end"][b] or abs(right - left) > 1e-4 * scale:
-                excluded += 1
-                continue
-            worst = max(worst, abs(grad[b, c] - (fd["plus"][b, c] - fd["minus"][b, c]) / (2 * hc)) / scale)
-    print(f"{name}: {m * ncol} perturbations, {excluded} excluded, worst {worst:.2e}")
-    return worst, excluded, m * ncol
 
 
 def flat_grad(ga, gx):
@@ -378,11 +286,8 @@ class Setup:
         self.warm = rng.uniform(-0.3, 0.3, (case.warm, m, nu))
         self._prepare(sim)
         x0 = sim.get_ode_state().cpu().numpy()
-        if ode_has_angle(self.cfg):
-            x0[:, -1] = np.clip(x0[:, -1], -2.5, 2.5)
-        if self.cfg.motor_kind in (K.MOTOR_SCIM, K.MOTOR_DFIM):  # a built-up rotor flux: the field frame is defined (DESIGN.md finding 3)
-            mag, ang = rng.uniform(0.2, 0.8, m), rng.uniform(-np.pi, np.pi, m)
-            x0[:, 3], x0[:, 4] = mag * np.cos(ang), mag * np.sin(ang)
+        clip_angle(self.cfg, x0)
+        build_up_flux(rng, self.cfg, x0)  # the field frame is defined (DESIGN.md finding 3)
         if case.envp:
             x0[:, 0] = 150.0  # outside the static-friction band: the speed-dependent load terms are live
         if case.omega0 is not None:

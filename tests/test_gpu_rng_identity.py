@@ -7,101 +7,25 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import load_golden, switched_config
+from gpu_helpers import DEAD3, SCIM_RANDOM, SWITCHED, _acts, _dev_actions, _random_cfg, _run, _same_outputs, torch_cuda  # noqa: F401
+from helpers import ROLLOUT_CASES
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import _random_actions, torch_cuda  # noqa: F401
-from test_gpu_rollout import CASES, _dev_actions, _mk
 
 pytestmark = pytest.mark.gpu
 
-DEAD3 = "pmsm_cc_rk4_dead3"
-SWITCHED = "switched_periodic"
-SCIM_RANDOM = "scim_random_init"
 CROSS_RESETS = ("pmsm_cc_rk4", "eesm_cc_rk4", "permex_cc_rk4")
-ALL = CASES + [DEAD3, SWITCHED, SCIM_RANDOM]
+ALL = ROLLOUT_CASES + [DEAD3, SWITCHED, SCIM_RANDOM]
 # Per-env blocks set from the host derive a constant initial state's reset observation on the device, which differs in the last bits from
 # the host-derived one of the shared-coefficient kernels for the induction motors (DESIGN.md §4); blocks made by an adoption use the latter.
 HOST_EXACT = [c for c in ALL if not c.startswith(("scim", "dfim"))]
-
-
-def _randomise(g, cfg):
-    """random initial states on omega and the first currents (induction motors: their flux limits come from the env's initializer, see
-    SCIM_RANDOM), and normal state noise on the first two states"""
-    init = [cfg.init_ode[j] for j in range(8)]
-    lim = np.array(g["meta"]["limits"])
-    n_ode = len(g["reset_ode"])
-    if cfg.motor_kind not in (K.MOTOR_SCIM, K.MOTOR_DFIM):
-        cfg.init_random = 1
-        for j in range(n_ode):
-            span = (0.2 * lim[0] if j == 0 else 0.3 * lim[2]) if j < 3 else 0.0
-            cfg.init_lo[j], cfg.init_hi[j] = init[j] - span, init[j] + span
-    if cfg.n_state_ops < K.MAX_STATE_OPS:
-        k = cfg.n_state_ops
-        cfg.n_state_ops = k + 1
-        cfg.sop_kind[k], cfg.sop_idx[k][0], cfg.sop_mask[k] = K.SOP_NOISE, K.NOISE_NORMAL, 0b11
-        cfg.sop_param[k][0], cfg.sop_param[k][1] = 0.0, 0.01
-
-
-def _cfg(name, n, dtype, seed=77, offset=12345):
-    """(golden or None, config) of a case with its random parts on"""
-    if name == SWITCHED:
-        kinds = [dict(kind=K.REF_WIENER, margin=(-0.5, 0.5), length=(2, 6)), dict(kind=K.REF_SINUS, length=(2, 6)),
-                 dict(kind=K.REF_STEP, amp=(0.05, 0.2), length=(2, 6)), dict(kind=K.REF_TRIANGULAR, length=(3, 7))]
-        cfg = switched_config(n, kinds, [0.25] * 4, (5, 12), seed=seed, dtype=dtype)
-        cfg.env_index_offset = offset
-        return load_golden("permex_sc_euler3"), cfg
-    if name == SCIM_RANDOM:
-        import gym_electric_motor_b200 as gem
-
-        cfg = gem.make("Cont-CC-SCIM-v0", num_envs=n, motor=dict(motor_initializer=dict(random_init="uniform"))).build_config()
-        assert cfg.init_im_valid == 1
-        cfg.dtype, cfg.seed, cfg.env_index_offset = dtype, seed, offset
-        return None, cfg
-    g, cfg = _mk(name.replace("_dead3", ""), n, dtype, K.LAYOUT_AOS)
-    if name == DEAD3:
-        cfg.dead_time_steps = 3
-    _randomise(g, cfg)  # (_mk already leaves the AC supply's phase random)
-    cfg.seed, cfg.env_index_offset = seed, offset
-    return g, cfg
-
-
-def _acts(rng, g, sim, steps):
-    if g is None:
-        return rng.uniform(-1, 1, size=(steps, sim.n, sim.n_act))
-    return _random_actions(rng, g, sim.n, steps)
-
-
-def _run(torch, sim, acts, mode, idx):
-    """outputs of envs idx over len(acts) steps: eager steps, one recorded rollout, or steps captured in a CUDA graph (device clock)"""
-    k = acts.shape[0]
-    if mode == "rollout":
-        o = sim.rollout(acts, record_every=1)
-        return [tuple(t[j][idx].clone() for t in o) for j in range(k)]
-    if mode == "graph":
-        sim.set_device_clock(True)
-        torch.cuda.synchronize()
-        graph, rec = torch.cuda.CUDAGraph(), []
-        with torch.cuda.graph(graph):
-            for j in range(k):
-                rec.append(tuple(t.clone() for t in sim.step(acts[j])))
-        graph.replay()
-        torch.cuda.synchronize()
-        return [tuple(t[idx] for t in r) for r in rec]
-    return [tuple(t[idx].clone() for t in sim.step(acts[j])) for j in range(k)]
-
-
-def _same(torch, out_a, out_b, what):
-    for k, (oa, ob) in enumerate(zip(out_a, out_b)):
-        for q, nm in enumerate(("obs", "ref", "reward", "terminated")):
-            assert torch.equal(oa[q], ob[q]), (what, nm, k)
 
 
 def _branch_pair(torch, name, dtype, m=120, n_a=301, n_b=403, k1=7, k2=12):
     """A (seed 77, offset 12345) and B (seed 5, offset 999, other N): A's envs src restored with their identities into B's envs dst"""
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg_a = _cfg(name, n_a, dtype)
-    _, cfg_b = _cfg(name, n_b, dtype, seed=5, offset=999)
+    g, cfg_a = _random_cfg(name, n_a, dtype)
+    _, cfg_b = _random_cfg(name, n_b, dtype, seed=5, offset=999)
     a, b = VectorSim(cfg_a), VectorSim(cfg_b)
     rng = np.random.default_rng(3)
     src, dst = rng.permutation(n_a)[:m], rng.permutation(n_b)[:m]
@@ -133,7 +57,7 @@ def test_per_env_blocks_of_the_shared_parameters_match_the_shared_kernels(torch_
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg = _cfg(name, 257, dtype)
+    g, cfg = _random_cfg(name, 257, dtype)
     a, b = VectorSim(cfg), VectorSim(cfg)
     if blocks == "host_blocks":
         b.set_env_params(np.tile(np.array(list(cfg.motor_param)), (b.n, 1)), np.tile(np.array(list(cfg.load_param)), (b.n, 1)))
@@ -143,8 +67,8 @@ def test_per_env_blocks_of_the_shared_parameters_match_the_shared_kernels(torch_
     assert torch.equal(ra[0], rb[0]) and torch.equal(ra[1], rb[1])
     acts = _dev_actions(torch, a, _acts(np.random.default_rng(1), g, a, 24))
     everyone = torch.arange(a.n, device=a.device)
-    _same(torch, _run(torch, a, acts[:12], "step", everyone), _run(torch, b, acts[:12], "step", everyone), "step")
-    _same(torch, _run(torch, a, acts[12:], "rollout", everyone), _run(torch, b, acts[12:], "rollout", everyone), "rollout")
+    _same_outputs(torch, _run(torch, a, acts[:12], "step", everyone), _run(torch, b, acts[:12], "step", everyone), "step")
+    _same_outputs(torch, _run(torch, a, acts[12:], "rollout", everyone), _run(torch, b, acts[12:], "rollout", everyone), "rollout")
     a.close()
     b.close()
 
@@ -159,7 +83,7 @@ def test_adopted_identity_replays_the_source(torch_cuda, name, dtype, mode):
     da, db = _same_actions(torch, g, a, b, src, dst, rng)
     out_a = _run(torch, a, da, mode, torch.as_tensor(src, device=a.device))
     out_b = _run(torch, b, db, mode, torch.as_tensor(dst, device=b.device))
-    _same(torch, out_a, out_b, (name, mode))
+    _same_outputs(torch, out_a, out_b, (name, mode))
     if name in CROSS_RESETS:
         assert sum(int(o[3].sum().item()) for o in out_a) > 0, "the case is meant to cross terminations + in-kernel resets after the restore"
     a.close()
@@ -176,7 +100,7 @@ def test_masked_reset_draws_with_the_identity(torch_cuda):
     s2, d2 = torch.as_tensor(src[::2], device=a.device), torch.as_tensor(dst[::2], device=b.device)
     assert torch.equal(oa[0][s2], ob[0][d2]) and torch.equal(oa[1][s2], ob[1][d2])
     da, db = _same_actions(torch, g, a, b, src, dst, rng, steps=8)
-    _same(torch, _run(torch, a, da, "step", torch.as_tensor(src, device=a.device)), _run(torch, b, db, "step", torch.as_tensor(dst, device=b.device)), "after")
+    _same_outputs(torch, _run(torch, a, da, "step", torch.as_tensor(src, device=a.device)), _run(torch, b, db, "step", torch.as_tensor(dst, device=b.device)), "after")
     a.close()
     b.close()
 
@@ -186,7 +110,7 @@ def test_fan_out_on_one_handle(torch_cuda):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    g, cfg = _cfg("pmsm_cc_rk4", 300, K.F32)
+    g, cfg = _random_cfg("pmsm_cc_rk4", 300, K.F32)
     h = VectorSim(cfg)
     rng = np.random.default_rng(9)
     h.reset()
@@ -222,7 +146,7 @@ def test_branch_of_a_branch_replays_the_original(torch_cuda, dtype):
     from gym_electric_motor_b200.vector_sim import VectorSim
 
     g, a, b, src, dst, rng = _branch_pair(torch, "pmsm_cc_rk4", dtype)
-    _, cfg_c = _cfg("pmsm_cc_rk4", 97, dtype, seed=11, offset=3)
+    _, cfg_c = _random_cfg("pmsm_cc_rk4", 97, dtype, seed=11, offset=3)
     c = VectorSim(cfg_c)
     c.reset()
     for x in _dev_actions(torch, c, _acts(rng, g, c, 4)):
@@ -238,7 +162,7 @@ def test_branch_of_a_branch_replays_the_original(torch_cuda, dtype):
     acts_c[:, cdst] = acts_a[:, src[:m]]
     out_a = _run(torch, a, _dev_actions(torch, a, acts_a), "step", torch.as_tensor(src[:m], device=a.device))
     out_c = _run(torch, c, _dev_actions(torch, c, acts_c), "step", torch.as_tensor(cdst, device=c.device))
-    _same(torch, out_a, out_c, "A -> B -> C")
+    _same_outputs(torch, out_a, out_c, "A -> B -> C")
     for s in (a, b, c):
         s.close()
 
@@ -249,7 +173,7 @@ def test_default_restore_returns_to_the_own_draws(torch_cuda):
     from gym_electric_motor_b200.vector_sim import VectorSim
 
     g, a, b, src, dst, rng = _branch_pair(torch, "pmsm_cc_rk4", K.F32)
-    b2 = VectorSim(_cfg("pmsm_cc_rk4", b.n, K.F32, seed=5, offset=999)[1])  # B's twin: the same clock, no identities adopted
+    b2 = VectorSim(_random_cfg("pmsm_cc_rk4", b.n, K.F32, seed=5, offset=999)[1])  # B's twin: the same clock, no identities adopted
     acts = _dev_actions(torch, b, _acts(rng, g, b, 36))
     b2.reset()
     for k in range(24):
@@ -262,7 +186,7 @@ def test_default_restore_returns_to_the_own_draws(torch_cuda):
     b.restore(snap, idx=ii)
     b2.restore(snap, idx=ii)
     everyone = torch.arange(b.n, device=b.device)
-    _same(torch, _run(torch, b, acts[24:], "step", everyone), _run(torch, b2, acts[24:], "step", everyone), "default restore")
+    _same_outputs(torch, _run(torch, b, acts[24:], "step", everyone), _run(torch, b2, acts[24:], "step", everyone), "default restore")
     for s in (a, b, b2):
         s.close()
 
@@ -273,13 +197,13 @@ def test_reseed_after_adoption_is_a_fresh_handle(torch_cuda):
 
     g, a, b, src, dst, rng = _branch_pair(torch, "pmsm_cc_rk4", K.F32)
     b.reseed(4242)
-    _, cfg_f = _cfg("pmsm_cc_rk4", b.n, K.F32, seed=4242, offset=999)
+    _, cfg_f = _random_cfg("pmsm_cc_rk4", b.n, K.F32, seed=4242, offset=999)
     f = VectorSim(cfg_f)
     acts = _dev_actions(torch, b, _acts(rng, g, b, 24))
     everyone = torch.arange(b.n, device=b.device)
     rb, rf = b.reset(), f.reset()
     assert torch.equal(rb[0], rf[0]) and torch.equal(rb[1], rf[1])
-    _same(torch, _run(torch, b, acts, "rollout", everyone), _run(torch, f, acts, "rollout", everyone), "reseed")
+    _same_outputs(torch, _run(torch, b, acts, "rollout", everyone), _run(torch, f, acts, "rollout", everyone), "reseed")
     assert np.array_equal(b.state_dict()["blob"], f.state_dict()["blob"])  # checkpoints work again
     for s in (a, b, f):
         s.close()
@@ -290,7 +214,7 @@ def test_clear_returns_every_env_to_its_own_draws(torch_cuda):
     from gym_electric_motor_b200.vector_sim import VectorSim
 
     g, a, b, src, dst, rng = _branch_pair(torch, "pmsm_cc_rk4", K.F64)
-    b2 = VectorSim(_cfg("pmsm_cc_rk4", b.n, K.F64, seed=5, offset=999)[1])  # B's twin: the same clock, the same states, its own identities
+    b2 = VectorSim(_random_cfg("pmsm_cc_rk4", b.n, K.F64, seed=5, offset=999)[1])  # B's twin: the same clock, the same states, its own identities
     b2.reset()
     for x in _dev_actions(torch, b2, _acts(rng, g, b2, 12)):
         b2.step(x)
@@ -298,7 +222,7 @@ def test_clear_returns_every_env_to_its_own_draws(torch_cuda):
     b.clear_rng_ids()
     acts = _dev_actions(torch, b, _acts(rng, g, b, 24))
     everyone = torch.arange(b.n, device=b.device)
-    _same(torch, _run(torch, b, acts, "step", everyone), _run(torch, b2, acts, "step", everyone), "clear")
+    _same_outputs(torch, _run(torch, b, acts, "step", everyone), _run(torch, b2, acts, "step", everyone), "clear")
     for s in (a, b, b2):
         s.close()
 
@@ -317,7 +241,7 @@ def test_refusals(torch_cuda):
             call()
     assert b._lib.gemb200_checkpoint_save(b._h, C.c_void_p(np.empty(b._lib.gemb200_checkpoint_size(b._h), np.uint8).ctypes.data)) == K.E_INVALID
     # SoA layout
-    _, cfg_s = _cfg("pmsm_cc_rk4", 64, K.F32)
+    _, cfg_s = _random_cfg("pmsm_cc_rk4", 64, K.F32)
     cfg_s.layout = K.LAYOUT_SOA
     s = VectorSim(cfg_s)
     snap = a.snapshot(src, rng=True)
@@ -325,7 +249,7 @@ def test_refusals(torch_cuda):
         s.restore(snap, idx=np.arange(8), rng="source")
     assert s._lib.gemb200_adopt_rng_ids(s._h, C.c_void_p(ids.data_ptr()), 8, None, None, 8, s._stream()) == K.E_INVALID
     # parameter draws on
-    _, cfg_d = _cfg("pmsm_cc_rk4", 64, K.F32)
+    _, cfg_d = _random_cfg("pmsm_cc_rk4", 64, K.F32)
     d = VectorSim(cfg_d)
     d.set_param_randomization([K.MP_R_S], [K.DIST_UNIFORM], [0.1], [0.2])
     assert d._lib.gemb200_adopt_rng_ids(d._h, C.c_void_p(ids.data_ptr()), 8, None, None, 8, d._stream()) == K.E_INVALID
@@ -350,8 +274,8 @@ def test_mpc_step_with_identities_matches_its_best_branch(torch_cuda):
     from gym_electric_motor_b200.vector_sim import VectorSim
 
     plants, cand, horizon = 16, 32, 6
-    g, cfg_p = _cfg("pmsm_cc_rk4", plants, K.F32)
-    _, cfg_m = _cfg("pmsm_cc_rk4", plants * cand, K.F32, seed=8, offset=0)
+    g, cfg_p = _random_cfg("pmsm_cc_rk4", plants, K.F32)
+    _, cfg_m = _random_cfg("pmsm_cc_rk4", plants * cand, K.F32, seed=8, offset=0)
     p, mdl = VectorSim(cfg_p), VectorSim(cfg_m)
     rng = np.random.default_rng(6)
     p.reset()

@@ -5,49 +5,15 @@ Oracle parity of the rollout path itself: test_rollout_matches_oracle."""
 import numpy as np
 import pytest
 
-from helpers import config_from_meta, load_golden, switched_config
+from gpu_helpers import _dev_actions, torch_cuda  # noqa: F401
+from helpers import ROLLOUT_CASES, _mk, _random_actions, config_from_meta, load_golden, switched_config
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import _random_actions, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-# plain / general instantiations, every motor family, the side state that lives outside the registers (switching states, dead-time
-# ring, RC / AC supply, flux observer, external speed profile position, switched generators)
-CASES = ["pmsm_cc_rk4", "pmsm_sc_polyload_rk4", "pmsm_fin_sc_rk4", "pmsm_fin_sc_rk4_interlock", "pmsm_cc_euler3", "synrm_cc_rk4", "eesm_cc_rk4",
-         "eesm_fin_cc_rk4", "scim_cc_rk4", "scim_fin_cc_interlock_rk4", "dfim_cc_rk4", "permex_cc_rk4", "series_cc_rk4", "shunt_cc_rk4", "extex_cc_rk4",
-         "permex_fin_sc_rc_interlock_rk4", "pmsm_cc_ac_rk4", "pmsm_cc_extspeed_rk4", "scim_sc_flux_cossin_dead1_rk4", "eesm_cc_rc_dq_dead1_rk4",
-         "pmsm_cc_cossin_rk4", "dfim_cc_flux_dq_rk4", "extex_fin_cc_interlock2_rk4", "dfim_fin_sc_interlock2_rk4"]
-
-
-def _mk(name, n, dtype, layout, ref_kind=K.REF_WIENER):
-    g = load_golden(name)
-    init = np.array(g["reset_ode"], dtype=float)
-    n_ode = len(init)
-    init[1:] = [0.7, -0.4, 0.02, 0.03, 0.3][: n_ode - 1] if g["meta"]["motor_class"] in ("SquirrelCageInductionMotor", "DoublyFedInductionMotor") else \
-        [0.9, -0.6, 0.5, 0.3][: n_ode - 1]
-    cfg = config_from_meta(g["meta"], n_envs=n, reset_ode=init, dtype=dtype, solver=None, ref_kind=ref_kind, autoreset=K.AUTORESET_SAME_STEP, seed=77,
-                           layout=layout)
-    for r in range(cfg.n_ref):
-        cfg.ref_margin_lo[r], cfg.ref_margin_hi[r] = -0.7, 0.7
-        cfg.ref_init_lo[r], cfg.ref_init_hi[r] = -0.7, 0.7
-        cfg.ref_len_lo[r], cfg.ref_len_hi[r] = 3, 9  # several sub-episode changes inside one rollout
-    cfg.env_index_offset = 12345
-    if cfg.supply_kind == K.SUPPLY_AC1:
-        cfg.supply_param[2] = 0.0
-    return g, cfg
-
-
-def _dev_actions(torch, sim, acts):
-    """[K, N, n_act] numpy -> device tensor in the sim's layout and action dtype"""
-    a = np.asarray(acts).reshape(acts.shape[0], sim.n, sim.n_act)
-    if sim.soa:
-        a = np.ascontiguousarray(a.transpose(0, 2, 1))
-    return torch.as_tensor(a, device=sim.device).to(sim.act_dtype).contiguous()
-
-
 @pytest.mark.parametrize("layout", [K.LAYOUT_AOS, K.LAYOUT_SOA], ids=["aos", "soa"])
 @pytest.mark.parametrize("dtype", [K.F32, K.F64], ids=["f32", "f64"])
-@pytest.mark.parametrize("name", CASES)
+@pytest.mark.parametrize("name", ROLLOUT_CASES)
 def test_rollout_is_bit_identical_to_repeated_steps(torch_cuda, name, dtype, layout):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim

@@ -13,8 +13,8 @@ import math
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
-from test_gpu_rollout_returns import ENV_IDS, _actions, _blob, _bits, _eq, _make, _next_steps, _same
+from fd_helpers import _cfg, build_up_flux, clip_angle, currents_off_zero, stencil, switching_states
+from gpu_helpers import ENV_IDS, _actions, _bits, _blob, _eq, _ext_env, _make, _next_steps, _same, torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -59,8 +59,6 @@ def test_primal_equals_recorded_rollout(torch_cuda, family, dtype, autoreset):
 
 
 def test_reference_feed(torch_cuda):
-    from test_gpu_rollout_returns import _ext_env
-
     torch = torch_cuda
     a_env, b_env = _ext_env(), _ext_env()
     sim = a_env.sim
@@ -179,15 +177,13 @@ def test_interlocked_finite_primal_and_fusion(torch_cuda, case, dtype, autoreset
     sims = [VectorSim(cfg) for _ in range(3)]
     for s_ in sims:
         s_.reset()
-    n_switch = {K.CONV_B6: 8, K.CONV_4QC: 4, K.CONV_2QC: 3, K.CONV_1QC: 2}
-    hi = np.array([n_switch[cfg.converter_kind[j]] for j in range(sims[0].n_act)])
     rng = np.random.default_rng(1)
     a_sim, b_sim, c_sim = sims
     for k in HORIZONS:
         if autoreset == "none":
             for s_ in sims:
                 s_.reset()
-        acts = torch.as_tensor(rng.integers(0, hi, (k, N, sims[0].n_act)), dtype=torch.int32, device="cuda").contiguous()
+        acts = torch.as_tensor(switching_states(rng, cfg, (k, N, sims[0].n_act)), dtype=torch.int32, device="cuda").contiguous()
         obs, ref, rew, term = a_sim.rollout(acts, record_every=1)
         (jx, ju), (o_b, r_b, w_b, t_b) = b_sim.rollout_jacobians(acts)
         assert ju is None and bool(torch.isfinite(jx).all())
@@ -282,41 +278,6 @@ def test_known_answer_linear_current_dynamics(torch_cuda, env_id):
 
 
 # ---------------------------------------------------------------------------------------------------------------- finite differences
-_KEEP = []
-
-
-def _profile(t, amplitude, frequency):
-    return amplitude * np.sin(2 * np.pi * frequency * t)
-
-
-def _cfg(env_id, n, dtype, solver=K.SOLVER_RK4, nsteps=1, load=None, supply=None, action_dq=0, til=None, til1=None, autoreset="none"):
-    import gym_electric_motor_b200 as gem
-
-    kw = {}
-    if load == "ext":  # a speed profile the load follows with its time constant (ExternalSpeedLoad)
-        kw["load"] = gem.physical_systems.ExternalSpeedLoad(speed_profile=_profile, speed_profile_kwargs=dict(amplitude=120.0, frequency=7.0),
-                                                          tau=1e-4, horizon_steps=2000)
-    env = gem.make(env_id, num_envs=n, dtype=dtype, autoreset=autoreset, seed=11, **kw)
-    _KEEP.append(env)  # the config points into the load's speed table, which the env owns
-    cfg = env.build_config()
-    cfg.solver_kind, cfg.solver_nsteps = solver, nsteps
-    if load == "const":
-        cfg.load_kind = K.LOAD_CONST_SPEED
-    elif load == "poly":
-        cfg.load_kind = K.LOAD_POLY_STATIC
-        cfg.load_param[K.LP_A], cfg.load_param[K.LP_B], cfg.load_param[K.LP_C] = 0.01, 0.02, 1e-4
-        cfg.load_param[K.LP_J_LOAD] = 1e-3
-    if supply == "ac1":
-        cfg.supply_kind, cfg.supply_param[0], cfg.supply_param[1], cfg.supply_param[2] = K.SUPPLY_AC1, 50.0, 0.3, 1.0
-    if action_dq:
-        cfg.action_dq = action_dq
-    if til is not None:
-        cfg.interlocking_time = til
-    if til1 is not None:
-        cfg.interlocking_time1 = til1
-    return cfg
-
-
 FD_CASES = {
     "permex-poly-rk4": ("Cont-CC-PermExDc-v0", dict(load="poly")),
     "series-poly-euler3": ("Cont-CC-SeriesDc-v0", dict(load="poly", solver=K.SOLVER_EULER, nsteps=3)),
@@ -360,53 +321,30 @@ def test_against_central_differences(torch_cuda, case):
     nx, nu = s0.jacobian_dims()
     rng = np.random.default_rng(5)
 
-    n_switch = {K.CONV_B6: 8, K.CONV_4QC: 4, K.CONV_2QC: 3, K.CONV_1QC: 2, K.CONV_NONE: 1}
-
     def draw_actions(k, n):
-        if s0.finite:  # a switching state per converter slot, within the slot's range
-            hi = np.array([n_switch[c0.converter_kind[j]] for j in range(s0.n_act)])
-            return torch.as_tensor(rng.integers(0, hi, (k, n, s0.n_act)), dtype=torch.int32, device="cuda").contiguous()
+        if s0.finite:
+            return torch.as_tensor(switching_states(rng, c0, (k, n, s0.n_act)), dtype=torch.int32, device="cuda").contiguous()
         # beyond +-1 on purpose: about a quarter of the legs clip, where the action derivative is 0
         return torch.as_tensor(rng.uniform(-1.3, 1.3, (k, n, s0.n_act)), dtype=torch.float64, device="cuda").contiguous()
 
     s0.rollout(draw_actions(3, m), record_every=1)
     x0 = s0.get_ode_state().cpu().numpy()
     has_eps = c0.motor_kind >= K.MOTOR_PMSM
-    if has_eps:
-        x0[:, -1] = np.clip(x0[:, -1], -2.5, 2.5)
-    if s0.finite:  # no current exactly at 0: there a leg waiting in its interlock state switches its voltage with the current's sign
-        cur = slice(1, c0.motor_kind >= K.MOTOR_PMSM and 3 or x0.shape[1])
-        x0[:, cur] += rng.choice([-1.0, 1.0], x0[:, cur].shape) * rng.uniform(0.5, 2.0, x0[:, cur].shape)
-    if c0.motor_kind in (K.MOTOR_SCIM, K.MOTOR_DFIM):  # a built-up rotor flux: near zero the field angle turns with any perturbation
-        mag, ang = rng.uniform(0.2, 0.8, m), rng.uniform(-np.pi, np.pi, m)
-        x0[:, 3], x0[:, 4] = mag * np.cos(ang), mag * np.sin(ang)
+    clip_angle(c0, x0)
+    currents_off_zero(rng, c0, x0)
+    build_up_flux(rng, c0, x0)
     a0 = draw_actions(1, m)[0].cpu().numpy()
     # finite converters: one step with other switching states first, the same on every copy of a base env (the switching state persists
     # across steps and decides, with an interlocking time, how many segments the linearised step has)
     a_prev = draw_actions(1, m)[0].cpu().numpy() if s0.finite else None
     ncol = nx + nu
-    reps = 2 * ncol + 1
-    n = m * reps
-    cfd = _cfg(env_id, n, "float64", **kw)
-    sim = VectorSim(cfd)
+    xs, acts, steps, reps = stencil(x0, a0[None], nu)
+    sim = VectorSim(_cfg(env_id, m * reps, "float64", **kw))
     sim.reset()
-    xs = np.repeat(x0, reps, axis=0)
-    acts = np.repeat(a0, reps, axis=0).astype(np.float64 if nu else np.int32)
-    steps = np.zeros(ncol)
-    for c in range(ncol):
-        if c < nx:
-            hc = 1e-6 * max(1.0, float(np.abs(x0[:, c]).max()))
-            xs[2 * c + 1::reps, c] += hc
-            xs[2 * c + 2::reps, c] -= hc
-        else:
-            hc = 1e-6
-            acts[2 * c + 1::reps, c - nx] += hc
-            acts[2 * c + 2::reps, c - nx] -= hc
-        steps[c] = hc
     if s0.finite:
         sim.step(torch.as_tensor(np.repeat(a_prev, reps, axis=0), device="cuda").contiguous())
     sim.set_ode_state(xs)
-    a_t = torch.as_tensor(acts[None], device="cuda").contiguous()
+    a_t = torch.as_tensor(acts, device="cuda").contiguous()
     (jx, ju), _ = sim.rollout_jacobians(a_t)
     x1 = sim.get_ode_state().cpu().numpy().reshape(m, reps, nx)
     jac = jx[0].cpu().numpy()[::reps]

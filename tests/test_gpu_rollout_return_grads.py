@@ -7,9 +7,8 @@
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
-from test_gpu_rollout_jacobians import _cfg
-from test_gpu_rollout_returns import ENV_IDS, _actions, _blob, _eq, _make, _next_steps
+from fd_helpers import _cfg, build_up_flux, clip_angle, compare_fd, stencil
+from gpu_helpers import ENV_IDS, _actions, _blob, _eq, _make, _next_steps, torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -130,54 +129,21 @@ def test_against_central_differences(torch_cuda, case):
     nx, nu, _ = s0.return_grad_dims()
     s0.rollout(torch.as_tensor(rng.uniform(-1.0, 1.0, (3, m, nu)), device="cuda").contiguous(), record_every=1)
     x0 = s0.get_ode_state().cpu().numpy()
-    has_eps = s0.cfg.motor_kind >= K.MOTOR_PMSM
-    if has_eps:
-        x0[:, -1] = np.clip(x0[:, -1], -2.5, 2.5)
-    if s0.cfg.motor_kind in (K.MOTOR_SCIM, K.MOTOR_DFIM):
-        mag, ang = rng.uniform(0.2, 0.8, m), rng.uniform(-np.pi, np.pi, m)
-        x0[:, 3], x0[:, 4] = mag * np.cos(ang), mag * np.sin(ang)
+    clip_angle(s0.cfg, x0)
+    build_up_flux(rng, s0.cfg, x0)
     a0 = rng.uniform(-1.3, 1.3, (k, m, nu))
     nref = s0.n_ref
     r0 = rng.uniform(-0.5, 0.5, (k, m, nref))
-    ncol = nx + k * nu
-    reps = 2 * ncol + 1
-    n = m * reps
-    sim = VectorSim(cfg(n))
+    xs, acts, steps, reps = stencil(x0, a0, nu)
+    sim = VectorSim(cfg(m * reps))
     sim.reset()
-    xs = np.repeat(x0, reps, axis=0)
-    acts = np.repeat(a0, reps, axis=1)
-    steps = np.zeros(ncol)
-    for c in range(ncol):
-        if c < nx:
-            hc = 1e-6 * max(1.0, float(np.abs(x0[:, c]).max()))
-            xs[2 * c + 1::reps, c] += hc
-            xs[2 * c + 2::reps, c] -= hc
-        else:
-            hc = 1e-6
-            kk, u = divmod(c - nx, nu)
-            acts[kk, 2 * c + 1::reps, u] += hc
-            acts[kk, 2 * c + 2::reps, u] -= hc
-        steps[c] = hc
     sim.set_ode_state(xs)
     refs = torch.as_tensor(np.repeat(r0, reps, axis=1), device="cuda").contiguous() if nref else None
     ret, end, _, ga, gx = sim.rollout_return_grads(torch.as_tensor(acts, device="cuda").contiguous(), gamma, references=refs)
     ret, end = ret.cpu().numpy().reshape(m, reps), end.cpu().numpy().reshape(m, reps)
     grad = np.concatenate([gx.cpu().numpy()[::reps], ga.cpu().numpy()[:, ::reps].transpose(1, 0, 2).reshape(m, -1)], axis=1)
-    skipped = total = 0
-    worst = 0.0
-    for b in range(m):
-        scale = max(np.abs(grad[b]).max(), 1e-12)
-        for c in range(ncol):
-            total += 1
-            ends = {end[b, 0], end[b, 2 * c + 1], end[b, 2 * c + 2]}
-            plus, minus, mid = ret[b, 2 * c + 1], ret[b, 2 * c + 2], ret[b, 0]
-            hc = steps[c]
-            right, left = (plus - mid) / hc, (mid - minus) / hc
-            if len(ends) > 1 or abs(right - left) > 1e-4 * scale:  # another branch on one side: a termination, a clip, |e| at 0
-                skipped += 1
-                continue
-            worst = max(worst, abs(grad[b, c] - (plus - minus) / (2 * hc)) / scale)
-    print(f"{case}: {total} perturbations, {skipped} excluded, worst {worst:.2e}")
+    fd = dict(target=ret[:, 0], end=end[:, 0], plus=ret[:, 1::2], minus=ret[:, 2::2], end_p=end[:, 1::2], end_m=end[:, 2::2], h=steps)
+    worst, skipped, total = compare_fd(case, grad, fd, 1e-5)
     assert skipped <= total // 5, (case, skipped, total)
     assert worst < 1e-5, (case, worst)
 

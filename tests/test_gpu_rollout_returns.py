@@ -5,43 +5,13 @@ both handles must end in the same persistent state (checkpoint blob, or snapshot
 import numpy as np
 import pytest
 
-from test_gpu_parity import torch_cuda  # noqa: F401
+from gpu_helpers import ENV_IDS, N, _actions, _bits, _blob, _eq, _ext_env, _make, _next_steps, _same, torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
 
-N = 300  # not a multiple of 128: the last block and its last warp are partly inactive
 HORIZONS = (64, 7, 1)
 DISCOUNTS = (1.0, 0.9, 0.0)
-
-ENV_IDS = {"permex": "Cont-CC-PermExDc-v0", "extex": "Cont-CC-ExtExDc-v0", "pmsm": "Cont-CC-PMSM-v0", "eesm": "Cont-CC-EESM-v0",
-           "scim": "Cont-CC-SCIM-v0", "dfim": "Cont-CC-DFIM-v0", "pmsm_finite": "Finite-CC-PMSM-v0"}
-
-
-def _make(family, dtype="float32", layout="aos", autoreset="same_step", seed=7, n=N, **kw):
-    import gym_electric_motor_b200 as gem
-
-    env = gem.make(ENV_IDS[family], num_envs=n, device="cuda", dtype=dtype, layout=layout, autoreset=autoreset, seed=seed, **kw)
-    env.reset()
-    return env
-
-
-def _actions(torch, env, k, seed=0):
-    """saturating actions with a per-env magnitude, constant in sign for stretches of 6 steps: currents leave their limits after a number
-    of steps that differs from env to env.  Finite B6: one active voltage vector per env, after a stretch of zero voltage of its own
-    length."""
-    sim = env.sim
-    rng = np.random.default_rng(seed)
-    lead = (k,) + sim._shape(sim.n_act)
-    if sim.finite:  # the zero vector (0) for each env's first 0 .. 8 steps staggers the steps at which the currents trip
-        a = np.array(np.broadcast_to(rng.integers(1, 7, size=lead[1:]), lead))
-        start = rng.integers(0, 9, size=lead[1:])
-        a[np.arange(k).reshape((k,) + (1,) * (len(lead) - 1)) < start] = 0
-        return torch.as_tensor(a, dtype=torch.int32, device="cuda").contiguous()
-    mag = rng.uniform(0.3, 1.0, size=(1,) + lead[1:])
-    a = np.repeat(rng.choice([-1.0, 1.0], size=((k + 5) // 6,) + lead[1:]), 6, axis=0)[:k] * mag
-    return torch.as_tensor(a, dtype=sim.dtype, device="cuda").contiguous()
-
 
 def _spec(torch, rew, term, discount):
     """the documented recurrence over recorded [K, N] rewards / terminations: w = 1, G = 0; G = G + (w * r_k) while not yet terminated;
@@ -60,29 +30,6 @@ def _spec(torch, rew, term, discount):
     return g, end
 
 
-def _bits(torch, x):
-    """bit pattern of a tensor (NaN-safe equality)"""
-    if x.dtype == torch.float32:
-        return x.contiguous().view(torch.int32)
-    if x.dtype == torch.float64:
-        return x.contiguous().view(torch.int64)
-    return x.contiguous().view(torch.uint8) if x.dtype == torch.bool else x
-
-
-def _eq(torch, a, b, what):
-    """bit equality"""
-    assert a.shape == b.shape and a.dtype == b.dtype, (what, a.shape, b.shape, a.dtype, b.dtype)
-    assert torch.equal(_bits(torch, a), _bits(torch, b)), (what, (a.double() - b.double()).abs().nan_to_num(1e300).max().item())
-
-
-def _same(torch, a, b, what):
-    """equal values (NaN equals NaN).  For the outputs of A's PLAIN kernel against B's general one: the instantiations agree value for
-    value but may differ in the sign of a zero (the equality the other rollout tests check with torch.equal)"""
-    assert a.shape == b.shape and a.dtype == b.dtype, (what, a.shape, b.shape, a.dtype, b.dtype)
-    ok = (a == b) | (torch.isnan(a) & torch.isnan(b)) if a.is_floating_point() else a == b
-    assert bool(ok.all()), (what, (a.double() - b.double()).abs().nan_to_num(1e300).max().item())
-
-
 def _pair(torch, a_env, b_env, acts, discount, refs=None, what=""):
     """A: recorded rollout, B: rollout_returns with the same actions; checks returns, end steps and the last outputs.  Returns B's
     returns and end steps."""
@@ -96,20 +43,6 @@ def _pair(torch, a_env, b_env, acts, discount, refs=None, what=""):
     _same(torch, o_b, obs[k - 1], (what, "obs"))
     _same(torch, r_b, ref[k - 1], (what, "ref"))
     return ret, end
-
-
-def _next_steps(torch, a_env, b_env, n=3, seed=99):
-    """the outputs of a few more steps on both handles: the same persistent state where no checkpoint can tell"""
-    acts = _actions(torch, a_env, n, seed=seed)
-    for j in range(n):
-        (o1, r1), w1, t1, _, _ = a_env.step(acts[j])
-        (o2, r2), w2, t2, _, _ = b_env.step(acts[j])
-        for name, x, y in (("obs", o1, o2), ("ref", r1, r2), ("reward", w1, w2), ("terminated", t1, t2)):
-            _same(torch, y, x, ("next step", j, name))
-
-
-def _blob(env):
-    return env.sim.state_dict()["blob"]
 
 
 def _assert_terminations(torch, end, k, what):
@@ -143,12 +76,6 @@ def test_returns_equal_recorded_rollout(torch_cuda, family, dtype, layout, autor
             assert a_env.sim.clock() == b_env.sim.clock(), what
     assert np.array_equal(_blob(a_env), _blob(b_env))
     _next_steps(torch, a_env, b_env)
-
-
-def _ext_env(layout="aos", dtype="float32", n=N):
-    from gym_electric_motor_b200.reference_generators import ExternalReferenceGenerator as Ext, MultipleReferenceGenerator
-
-    return _make("pmsm", dtype, layout, n=n, reference_generator=MultipleReferenceGenerator([Ext("i_sd"), Ext("i_sq")]))
 
 
 @pytest.mark.parametrize("layout", ["aos", "soa"])

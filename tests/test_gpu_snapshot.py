@@ -8,12 +8,12 @@ import pytest
 
 from helpers import switched_config
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import _random_actions, torch_cuda  # noqa: F401
-from test_gpu_rollout import CASES, _dev_actions, _mk
+from gpu_helpers import _dev_actions, torch_cuda  # noqa: F401
+from helpers import ROLLOUT_CASES, _mk, _random_actions
 
 pytestmark = pytest.mark.gpu
 
-DEAD3 = "pmsm_cc_rk4_dead3"  # every configuration in CASES has a dead time of 0 or 1: a ring of 1 cannot show a rotation error
+DEAD3 = "pmsm_cc_rk4_dead3"  # every configuration in ROLLOUT_CASES has a dead time of 0 or 1: a ring of 1 cannot show a rotation error
 
 
 def _cfg(name, n, dtype, layout, deterministic, seed=77, offset=12345):
@@ -71,7 +71,7 @@ def _branch(torch, name, dtype, layout, deterministic):
 
 @pytest.mark.parametrize("deterministic", [True, False], ids=["const", "wiener"])
 @pytest.mark.parametrize("dtype", [K.F32, K.F64], ids=["f32", "f64"])
-@pytest.mark.parametrize("name", CASES + [DEAD3])
+@pytest.mark.parametrize("name", ROLLOUT_CASES + [DEAD3])
 def test_branch_continues_like_its_source(torch_cuda, name, dtype, deterministic):
     out_a, out_b, n_term = _branch(torch_cuda, name, dtype, K.LAYOUT_AOS, deterministic)
     torch = torch_cuda

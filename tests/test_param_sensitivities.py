@@ -11,7 +11,7 @@ import torch
 
 import gym_electric_motor_b200 as gem
 from gym_electric_motor_b200 import _cabi as K
-from test_reference_feed import no_launch  # noqa: F401
+from helpers import NoLaunchSim, no_launch  # noqa: F401
 
 N = 6
 MOTOR_IDS = {K.MOTOR_PERMEX_DC: "Cont-CC-PermExDc-v0", K.MOTOR_SERIES_DC: "Cont-CC-SeriesDc-v0", K.MOTOR_SHUNT_DC: "Cont-CC-ShuntDc-v0",
@@ -209,7 +209,6 @@ def test_param_names(no_launch):
         env.rollout_param_sensitivities(acts, ["p"])
     with pytest.raises(KeyError):
         env.rollout_param_sensitivities(acts, ["q"])
-    from test_reference_feed import NoLaunchSim
 
     cfg = env.build_config()
     cfg.dead_time_steps = 1

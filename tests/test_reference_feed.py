@@ -10,43 +10,9 @@ import torch
 
 import gym_electric_motor_b200 as gem
 from gym_electric_motor_b200 import _cabi as K
-from gym_electric_motor_b200.vector_sim import VectorSim
+from helpers import _env, no_launch  # noqa: F401
 
-
-class _NoLaunch:
-    def __getattr__(self, name):
-        raise AssertionError(f"{name} was called: a bad reference feed must be refused before any launch")
-
-
-class NoLaunchSim(VectorSim):
-    """VectorSim on the CPU device whose library calls fail: every check of a feed runs, no launch does"""
-
-    def __init__(self, cfg, reuse_outputs=True):
-        d = [C.c_int32() for _ in range(4)]
-        K.check(K.load_library().gemb200_query_dims(C.byref(cfg), *[C.byref(x) for x in d]), "gemb200_query_dims")
-        self.n_state, self.n_ode, self.n_act, self.n_ref = [x.value for x in d]
-        self.cfg, self.n, self.finite = cfg, int(cfg.n_envs), bool(cfg.finite)
-        self.soa = cfg.layout == K.LAYOUT_SOA
-        self.dtype = torch.float32 if cfg.dtype == K.F32 else torch.float64
-        self.act_dtype = torch.int32 if self.finite else self.dtype
-        self.device = torch.device("cpu")
-        self._lib, self._h, self._reuse, self._out = _NoLaunch(), None, reuse_outputs, None
-
-
-@pytest.fixture
-def no_launch(monkeypatch):
-    import gym_electric_motor_b200.vector_sim as vs
-
-    monkeypatch.setattr(vs, "VectorSim", NoLaunchSim)
-
-
-N = 6
-
-
-def _env(**kw):
-    rg = gem.reference_generators.MultipleReferenceGenerator([gem.reference_generators.ExternalReferenceGenerator("i_sd"),
-                                                              gem.reference_generators.ExternalReferenceGenerator("i_sq")])
-    return gem.make("Cont-CC-PMSM-v0", num_envs=N, reference_generator=rg, dtype="float32", **kw)
+N = 6  # the envs of helpers._env
 
 
 def test_rollout_feed_argument_checks(no_launch):

@@ -1,4 +1,4 @@
-"""The oracle central-difference harness of test_gpu_return_grads_oracle.py against a closed form, without a GPU.
+"""The oracle central-difference harness of fd_helpers.py (used by test_gpu_return_grads_oracle.py) against a closed form, without a GPU.
 
 PMSM at constant speed, RK4 with one step per tau, continuous B6 bridge with actions inside the clip range, constant references on i_sd and
 i_sq and reward exponent 2, no constraint hit: the step is affine in (x, a),
@@ -10,7 +10,7 @@ import math
 
 import numpy as np
 
-from test_gpu_return_grads_oracle import oracle_fd
+from fd_helpers import oracle_fd
 from gym_electric_motor_b200 import _cabi as K
 
 

@@ -10,7 +10,7 @@ import torch
 
 import gym_electric_motor_b200 as gem
 from gym_electric_motor_b200 import _cabi as K
-from test_reference_feed import _env, no_launch  # noqa: F401
+from helpers import _env, no_launch  # noqa: F401
 
 N = 6
 

@@ -4,7 +4,6 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
 from helpers import *
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import DeviceAdapter
 from oracle.gem_oracle import Oracle
 g = load_golden("pmsm_cc_rk4")
 n = 600

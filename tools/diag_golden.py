@@ -5,7 +5,6 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
 from helpers import *
 from gym_electric_motor_b200 import _cabi as K
-from test_gpu_parity import DeviceAdapter
 
 for name in sys.argv[1:]:
     g = load_golden(name)
