@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <new>
 #include <limits>
 #include <string>
@@ -678,6 +679,21 @@ static int tick_clock(gemb200_handle* h, uint32_t d_call, uint32_t d_step, cudaS
   return GEMB200_OK;
 }
 
+// Caller device buffers of a launch (gemb200.h, "Alignment"; DESIGN.md §3): each pointer must be aligned to its element size, and the fp32
+// row-per-env reference output of 2 or 4 slots to the float2 / float4 the step and rollout kernels store per env (resets too, so that one
+// buffer serves every call).  A misaligned buffer would end in a misaligned-address fault that takes the CUDA context with it, so the
+// entry points refuse it before they launch or advance the clock.  NULL (an output not requested) passes.
+struct IoBuf { const char* name; const void* ptr; size_t align; };
+static int check_io(std::initializer_list<IoBuf> bufs) {
+  for (const IoBuf& b : bufs)
+    if (reinterpret_cast<uintptr_t>(b.ptr) % b.align)
+      return fail(GEMB200_E_INVALID, std::string(b.name) + " is not aligned to " + std::to_string(b.align) + " bytes");
+  return GEMB200_OK;
+}
+static size_t ref_align(const gemb200_handle* h) {
+  return h->rsz == 4 && h->cfg.layout == GEMB200_LAYOUT_AOS && (h->n_ref == 2 || h->n_ref == 4) ? 4 * (size_t)h->n_ref : (size_t)h->rsz;
+}
+
 // One launch over envs [begin, end) (end < 0: all).  new_call: this launch starts a new API call (fresh RNG call ids);
 // the chunks of one pipelined host step share them.  roll > 0: `roll` fused steps (rollout_kernel) whose call ids, step clock and
 // dead-time ring positions are exactly those of `roll` consecutive single-step calls; outputs every `every` steps (0: last only).
@@ -690,6 +706,11 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
                    int begin = 0, int end = -1, bool new_call = true, int roll = 0, int every = 0, const void* feed = nullptr,
                    void* ret = nullptr, int32_t* ret_end = nullptr, double discount = 1.0, const TanOut* tan = nullptr) {
   if (!action) return fail(GEMB200_E_INVALID, "action is NULL");
+  const size_t rsz = h->rsz;
+  if (int rc = check_io({{"action", action, h->cfg.finite ? sizeof(int32_t) : rsz}, {"obs_out", obs, rsz},
+                         {"ref_out", h->n_ref ? ref : nullptr, ref_align(h)}, {"reward_out", rew, rsz}, {"references", feed, rsz},
+                         {"return_out", ret, rsz}, {"end_step_out", ret_end, sizeof(int32_t)}}))
+    return rc;
   const uint64_t ksteps = roll > 0 ? (uint64_t)roll : 1;
   const bool dev_clock = h->dev_clock;
   if (dev_clock && (!new_call || begin != 0 || (end >= 0 && end != h->cfg.n_envs)))
@@ -722,6 +743,7 @@ static int do_step(gemb200_handle* h, const void* action, void* obs, void* ref, 
 }
 
 static int do_reset(gemb200_handle* h, const uint8_t* mask, void* obs, void* ref, cudaStream_t st) {
+  if (int rc = check_io({{"obs_out", obs, (size_t)h->rsz}, {"ref_out", h->n_ref ? ref : nullptr, ref_align(h)}})) return rc;
   const bool dev_clock = h->dev_clock;
   if (!dev_clock) h->gstep += 1;
   const cudaError_t e = with_params(h, [&](auto& p) {
@@ -1061,6 +1083,7 @@ int gemb200_rollout_jacobians(gemb200_handle* h, const void* actions, const void
   if (const char* why = jacobian_refusal(&h->cfg)) return fail(GEMB200_E_INVALID, why);
   if (!jac_x_out) return fail(GEMB200_E_INVALID, "jac_x_out is NULL");
   if (int rc = check_rollout(h, n_steps, references)) return rc;
+  if (int rc = check_io({{"jac_x_out", jac_x_out, (size_t)h->rsz}, {"jac_u_out", jac_u_out, (size_t)h->rsz}})) return rc;
   const JacOut jo{jac_x_out, h->cfg.finite ? nullptr : jac_u_out, h->cfg.finite ? 0 : h->n_act};
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
@@ -1082,6 +1105,9 @@ int gemb200_rollout_return_grads(gemb200_handle* h, const void* actions, const v
   const uint64_t words = (uint64_t)(d.n_ode * (d.n_ode + d.n_act) + d.n_ode + d.n_act);
   const uint64_t need = (uint64_t)n_steps * (uint64_t)h->cfg.n_envs * words * (uint64_t)h->rsz;
   if (workspace_bytes < need) return fail(GEMB200_E_INVALID, "workspace too small: it needs n_steps * n_envs * ws_words * sizeof(real) bytes (gemb200_query_return_grad_dims)");
+  const size_t rsz = h->rsz;
+  if (int rc = check_io({{"value_grad", value_grad, rsz}, {"workspace", workspace, rsz}, {"grad_a_out", grad_a_out, rsz}, {"grad_x0_out", grad_x0_out, rsz}}))
+    return rc;
   GradOut go{};
   go.ws = workspace; go.grad_a = grad_a_out; go.grad_x0 = grad_x0_out; go.value_grad = value_grad; go.nu = h->n_act;
   {  // the state-vector entry behind every reward term, in fill_params' order of the terms
@@ -1109,6 +1135,7 @@ int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const voi
     return fail(GEMB200_E_INVALID, "parameter sensitivities: parameter draws at resets are on, the parameters would change inside the launch (DESIGN.md §7)");
   if (!sens_io) return fail(GEMB200_E_INVALID, "sens_io is NULL");
   if (int rc = check_rollout(h, n_steps, references)) return rc;
+  if (int rc = check_io({{"sens_io", sens_io, (size_t)h->rsz}, {"sens_out", sens_out, (size_t)h->rsz}})) return rc;
   PsOut po{};
   po.sio = sens_io; po.sout = sens_out; po.np = n_p;
   for (int a = 0; a < n_p; ++a) po.slot[a] = slots[a];
@@ -1357,6 +1384,8 @@ int gemb200_bind_peers(gemb200_handle* h, int32_t n_dst, const int64_t* dst_delt
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   if (n_dst < 0 || n_dst > 8 || (n_dst > 0 && !dst_delta)) return fail(GEMB200_E_INVALID, "n_dst must be in [0, 8]");
   if (n_dst > 0 && h->cfg.layout != GEMB200_LAYOUT_AOS) return fail(GEMB200_E_INVALID, "peer destinations need the row-per-env (AoS) layout");
+  for (int d = 0; d < n_dst; ++d)  // the stores land at the caller's pointers + delta: a multiple of 16 keeps every pointer's alignment
+    if (dst_delta[d] % 16) return fail(GEMB200_E_INVALID, "dst_delta[" + std::to_string(d) + "] is not a multiple of 16 bytes");
   h->n_dst = n_dst;
   for (int d = 0; d < n_dst; ++d) h->dst_delta[d] = dst_delta[d];
   apply_mode(h);

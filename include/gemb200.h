@@ -282,6 +282,14 @@ int gemb200_query_dims(const gemb200_config* cfg, int32_t* n_state, int32_t* n_o
 int gemb200_create(const gemb200_config* cfg, gemb200_handle** out);
 int gemb200_destroy(gemb200_handle* h);
 
+/* Alignment.  Every device buffer a caller passes to gemb200_reset, gemb200_step, the gemb200_rollout* calls (returns, Jacobians, return
+ * gradients and parameter sensitivities included) must be aligned to its element size: 4 bytes for float / int32, 8 for double, 1 for
+ * uint8.  The fp32 row-per-env reference output (ref_out) is stored as one 8-byte vector per env with 2 reference slots and one 16-byte
+ * vector with 4, so it needs 8 or 16 bytes.  These calls return GEMB200_E_INVALID for a misaligned buffer, naming it, before they launch
+ * anything or advance the clock; NULL outputs are not checked.  gemb200_bind_peers requires every delta to be a multiple of 16 bytes,
+ * so that the peer destinations keep the alignment of the caller's buffers.  cudaMalloc'd buffers and the slices [k] of a contiguous
+ * [K][N][..] tensor satisfy the rule; a sub-buffer of a packed allocation need not. */
+
 /* ElectricMotorEnvironment.reset (core.py:300-319) -> SCMLSystem.reset (physical_systems.py:256-287, :527-561,
  * :659-693, :816-847) + ReferenceGenerator.reset.  reset_mask: device uint8[N] (non-zero = reset) or NULL for all.
  * obs_out/ref_out (device, layout per cfg, element type per cfg->dtype) may be NULL. */

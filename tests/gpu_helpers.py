@@ -20,6 +20,29 @@ def torch_cuda():
     return torch
 
 
+# ------------------------------------------------------------------------------------------------------------ launch shapes
+def launch_block(n, sms):
+    """threads per block of a step / rollout launch over n envs on a device with `sms` SMs: pick_block in csrc/gemb200_launch.cuh (128,
+    halved while the grid would have fewer than 8 blocks per SM, down to 32)"""
+    block = 128
+    while block > 32 and (n + block - 1) // block < sms * 8:
+        block //= 2
+    return block
+
+
+def launch_sizes():
+    """the batch sizes of the launch-shape tests, from the SM count S of cuda:0 (S = 132 on an H100 SXM: 67 617, 135 205, 67 584, 405 581):
+    N64 = 512 S + 33 launches 64-thread blocks, the last one a full warp and a warp with 1 env; N128 = 1024 S + 37 launches 128-thread
+    blocks, the last one a full warp, a warp with 5 envs and two empty warps; PF = 512 S is the step kernel's L2 prefetch distance (both
+    sizes exceed it); NHOST = 3072 S + 77: the pipelined host step's chunks launch 64 threads, a full-batch device step 128"""
+    import torch
+
+    s = torch.cuda.get_device_properties(0).multi_processor_count
+    sizes = dict(S=s, N64=512 * s + 33, N128=1024 * s + 37, PF=512 * s, NHOST=3072 * s + 77)
+    assert (launch_block(N, s), launch_block(sizes["N64"], s), launch_block(sizes["N128"], s), launch_block(sizes["NHOST"], s)) == (32, 64, 128, 128)
+    return sizes
+
+
 # ------------------------------------------------------------------------------------------------------------ env makers and actions
 N = 300  # not a multiple of 128: the last block and its last warp are partly inactive
 
@@ -187,6 +210,7 @@ _MOTOR_SLOTS = {  # parameters drawn per reset, +-20 % around the configuration'
     K.MOTOR_PMSM: (K.MP_R_S, K.MP_L_D, K.MP_L_Q, K.MP_PSI_P, K.MP_J_ROTOR),
     K.MOTOR_EESM: (K.MP_R_S, K.MP_L_D, K.MP_L_Q, K.MP_R_E, K.MP_J_ROTOR),
     K.MOTOR_PERMEX_DC: (K.MP_R_A, K.MP_L_A, K.MP_PSI_E, K.MP_J_ROTOR),
+    K.MOTOR_EXTEX_DC: (K.MP_R_A, K.MP_L_A, K.MP_R_E, K.MP_L_E, K.MP_J_ROTOR),
     K.MOTOR_SCIM: (K.MP_J_ROTOR,),
     K.MOTOR_DFIM: (K.MP_R_S, K.MP_L_M, K.MP_J_ROTOR),
 }
@@ -203,6 +227,18 @@ def _draws(cfg):
 _TANGENT_ENVP_ARG = {"jacobian_kernel": 4, "param_sens_kernel": 4, "return_grad_kernel": 3}
 
 
+def _mode(name):
+    """(kernel, mode) of a step, rollout, Jacobian, parameter-sensitivity or return-gradient kernel name, or None for any other kernel"""
+    m = re.search(r"(return_grad_kernel|param_sens_kernel|jacobian_kernel|step_kernel|rollout_kernel)<([^>]*)>", name)
+    if not m:
+        return None
+    kernel = m.group(1)
+    on = [a.strip() in ("true", "(bool)1", "1") for a in m.group(2).split(",")]
+    if kernel in ("step_kernel", "rollout_kernel"):
+        return kernel, "PLAIN" if on[5] else ("ENVP" if on[7] else "general")
+    return kernel, "ENVP" if on[_TANGENT_ENVP_ARG[kernel]] else "shared"
+
+
 def _kernels(torch, fn):
     """(kernel, mode) of every step, rollout, Jacobian, parameter-sensitivity and return-gradient kernel that fn() launches, in launch
     order, read from the kernel names torch.profiler records.  Step and rollout kernels: "PLAIN", "ENVP" or "general"; the tangent
@@ -212,15 +248,26 @@ def _kernels(torch, fn):
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
         torch.cuda.synchronize()
+    return [km for km in (_mode(e.name) for e in prof.events()) if km]
+
+
+def _launches(torch, fn, tmp_path):
+    """(kernel, mode, threads per block, blocks) of every kernel of `_kernels` that fn() launches, in launch order, read from the "block" and
+    "grid" fields of the kernel events in the exported profiler trace"""
+    import json
+
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    path = tmp_path / "trace.json"
+    prof.export_chrome_trace(str(path))
     out = []
-    for e in prof.events():
-        m = re.search(r"(return_grad_kernel|param_sens_kernel|jacobian_kernel|step_kernel|rollout_kernel)<([^>]*)>", e.name)
-        if not m:
-            continue
-        kernel = m.group(1)
-        on = [a.strip() in ("true", "(bool)1", "1") for a in m.group(2).split(",")]
-        if kernel in ("step_kernel", "rollout_kernel"):
-            out.append((kernel, "PLAIN" if on[5] else ("ENVP" if on[7] else "general")))
-        else:
-            out.append((kernel, "ENVP" if on[_TANGENT_ENVP_ARG[kernel]] else "shared"))
+    for e in sorted(json.loads(path.read_text())["traceEvents"], key=lambda e: e.get("ts", 0)):
+        km = _mode(e.get("name", "")) if e.get("cat") == "kernel" else None
+        if km:
+            args = e.get("args", {})
+            assert "block" in args and "grid" in args, ("the trace has no launch shape for", e["name"][:80], sorted(args))
+            out.append(km + (int(args["block"][0]), int(args["grid"][0])))
     return out

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 from gym_electric_motor_b200 import _cabi as K
+from helpers import WEAK_DQ_PAIRS, fold_weak_dq
 
 pytestmark = pytest.mark.gpu
 
@@ -59,7 +60,7 @@ def test_device_matches_oracle_for_host_built_config(oracle_lib, case):
     # still (numerically) zero after the reset — in the reference itself (DESIGN.md finding 3; same treatment as
     # test_gpu_parity.test_device_reproduces_reference_trajectory): there the dq pairs are compared through their magnitude and the
     # reward (which sees i_sd / i_sq in current-control envs) is not compared.
-    dq_pairs = {K.MOTOR_SCIM: ((5, 6), (10, 11)), K.MOTOR_DFIM: ((5, 6), (10, 11), (15, 16), (20, 21))}.get(cfg.motor_kind, ())
+    dq_pairs = WEAK_DQ_PAIRS.get(cfg.motor_kind, ())
     for k in range(12):
         if hasattr(sp, "low"):
             a = rng.uniform(sp.low, sp.high, size=(n, len(sp.low)))
@@ -75,11 +76,7 @@ def test_device_matches_oracle_for_host_built_config(oracle_lib, case):
         weak = np.zeros(n, dtype=bool)
         if dq_pairs:
             weak = np.hypot(psi[:, 0], psi[:, 1]) < 1e-3
-            for arr in (d_obs, o_obs):
-                for a_, b_ in dq_pairs:
-                    if b_ < arr.shape[1]:
-                        arr[weak, a_] = np.hypot(arr[weak, a_], arr[weak, b_])
-                        arr[weak, b_] = 0.0
+            fold_weak_dq(dq_pairs, weak, d_obs, o_obs)
         assert np.abs(d_obs - o_obs).max() < tol, (case, k)
         assert np.abs(d[1].double().cpu().numpy() - o[1]).max() < tol, (case, k)
         assert np.abs(d[2].double().cpu().numpy() - o[2])[~weak].max(initial=0.0) < 10 * tol, (case, k)

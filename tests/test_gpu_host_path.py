@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 
 from gym_electric_motor_b200 import _cabi as K
-from gpu_helpers import _draws, torch_cuda  # noqa: F401
+from gpu_helpers import _draws, launch_sizes, torch_cuda  # noqa: F401
 from helpers import _mk
 
 pytestmark = pytest.mark.gpu
@@ -168,7 +168,10 @@ def _pipeline_cases():
     for n in SIZES:
         out += [pytest.param("bench", b, K.F32, n, id=f"{b}-{n}") for b in BENCH]
     out += [pytest.param("bench", "scim", K.F32, n, id=f"scim-{n}") for n in SIZES[-2:]]
-    for n in SMALL:
+    # NHOST (gpu_helpers.launch_sizes): the chunks launch 64-thread blocks while the twin's full-batch step launches 128, so the two sides
+    # run one configuration at two launch shapes
+    out += [pytest.param("bench", b, K.F32, "NHOST", id=f"{b}-NHOST") for b in BENCH]
+    for n in SMALL + ["NHOST"]:
         out += [pytest.param("golden", g, K.F32, n, id=f"{g}-{n}") for g in GENERAL]
         out += [pytest.param("golden", g, K.F64, n, id=f"{g}-f64-{n}") for g in FP64]
         out += [pytest.param("draws", "pmsm_cc_rk4", K.F32, n, id=f"envp_draws-{n}"), pytest.param("rng_ids", "pmsm_cc_rk4", K.F32, n, id=f"rng_ids-{n}")]
@@ -185,6 +188,7 @@ def test_step_host_equals_device_step(torch_cuda, kind, name, dtype, n):
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
+    n = launch_sizes()[n] if n == "NHOST" else n
     cfg, act, _ = _case("bench" if kind == "bench" else "golden", name, dtype, n)
     host, twin = VectorSim(cfg), VectorSim(cfg)
     rng = np.random.default_rng(n)

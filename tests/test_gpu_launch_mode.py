@@ -1,6 +1,6 @@
 """Which kernel and instantiation a handle launches: the step / rollout instantiation as its per-env parameters, draws, RNG identities and
 peer destinations come and go, and the kernels of a reference feed, of Jacobians, of parameter sensitivities, of return gradients and of
-discounted returns.
+discounted returns; and the block size of step and rollout launches at the batch sizes of the launch-shape tests.
 
 The PLAIN, general and ENVP instantiations give bit-identical results (DESIGN.md §2), so no output test notices a handle that takes the
 wrong one; only its speed does (DESIGN.md §4: shared coefficients against per-env blocks).  These tests read the kernel and its
@@ -11,7 +11,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from gpu_helpers import _kernels, torch_cuda  # noqa: F401
+from gpu_helpers import N as N_SMALL, _kernels, _launches, launch_block, launch_sizes, torch_cuda  # noqa: F401
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -169,6 +169,55 @@ def test_device_clock_and_cuda_graph(torch_cuda, dtype):
         terminated += int(t_h.sum())
     assert terminated > 0
     assert host.sim.clock() == dev.sim.clock() == cap.sim.clock()
+
+
+def test_launch_blocks(torch_cuda, tmp_path):
+    """the block size of the step and rollout launches (pick_block): 32, 64 and 128 threads at N = 300, N64 and N128 (gpu_helpers.launch_sizes)
+    for the PLAIN shape, a general instantiation (state wrappers widen its rows) and per-env blocks (ENVP); and the pipelined host step at
+    NHOST: four chunks of 64-thread blocks, while the twin's full-batch device step launches 128.  test_gpu_launch_shape relies on these
+    shapes: if pick_block changes, this test fails instead of letting those tests quietly run one-warp blocks."""
+    torch = torch_cuda
+    import gym_electric_motor_b200 as gem
+    from helpers import ENV_PARAM_CASES
+
+    sz = launch_sizes()
+    s = sz["S"]
+
+    def general(n):
+        env_id, kw = ENV_PARAM_CASES["cc-scim-observer-dq"]()
+        env = gem.make(env_id, num_envs=n, device="cuda", dtype="float32", autoreset="same_step", seed=0, **kw)
+        env.reset()
+        return env
+
+    def envp(n):
+        env = _make(n)
+        r_s = float(env.sim.cfg.motor_param[K.MP_R_S])
+        env.set_env_parameters(motor_parameter={"r_s": r_s * np.linspace(0.9, 1.1, n)})
+        return env
+
+    _launches(torch, lambda: None, tmp_path)  # the profiler's first session pays its set-up
+    seen, want = [], []
+    for mode, mk in (("PLAIN", _make), ("general", general), ("ENVP", envp)):
+        for n in (N_SMALL, sz["N64"], sz["N128"]):
+            env = mk(n)
+            n_act = env.sim.n_act
+            acts = torch.zeros(2, n, n_act, device="cuda")
+            got = _launches(torch, lambda: (env.step(acts[0]), env.rollout(acts, record_every=1)), tmp_path)
+            block = launch_block(n, s)
+            seen.append((mode, n, got))
+            want.append((mode, n, [(k, mode, block, (n + block - 1) // block) for k in ("step_kernel", "rollout_kernel")]))
+            env.close()
+    assert [launch_block(n, s) for n in (N_SMALL, sz["N64"], sz["N128"])] == [32, 64, 128]
+    assert seen == want
+    # the pipelined host step: four chunks of whole 256-env blocks, one launch each, against the twin's one launch over all envs
+    n = sz["NHOST"]
+    host, twin = _make(n), _make(n)
+    a = np.zeros((n, 3), dtype=np.float32)
+    per = ((n + 3) // 4 + 255) // 256 * 256
+    chunks = [min(per, n - b) for b in range(0, n, per)]
+    got = _launches(torch, lambda: (host.sim.step_host(a), twin.sim.step(torch.zeros(n, 3, device="cuda"))), tmp_path)
+    assert [launch_block(c, s) for c in chunks] == [64] * 4
+    assert got == [("step_kernel", "PLAIN", 64, (c + 63) // 64) for c in chunks] + [("step_kernel", "PLAIN", 128, (n + 127) // 128)]
 
 
 def test_return_grad_launch_modes(torch_cuda):

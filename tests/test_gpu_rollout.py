@@ -5,8 +5,8 @@ Oracle parity of the rollout path itself: test_rollout_matches_oracle."""
 import numpy as np
 import pytest
 
-from gpu_helpers import _dev_actions, torch_cuda  # noqa: F401
-from helpers import ROLLOUT_CASES, _mk, _random_actions, config_from_meta, load_golden, switched_config
+from gpu_helpers import _dev_actions, launch_sizes, torch_cuda  # noqa: F401
+from helpers import ROLLOUT_CASES, WEAK_DQ_PAIRS, _mk, _random_actions, _tol, config_from_meta, fold_weak_dq, load_golden, switched_config
 from gym_electric_motor_b200 import _cabi as K
 
 pytestmark = pytest.mark.gpu
@@ -89,14 +89,24 @@ def test_rollout_with_switched_and_periodic_generators(torch_cuda, case):
     assert np.array_equal(a.state_dict()["blob"], b.state_dict()["blob"])
 
 
-@pytest.mark.parametrize("dtype,tol", [(K.F64, 1e-9), (K.F32, 1e-5)], ids=["f64", "f32"])
-@pytest.mark.parametrize("name", ["pmsm_cc_rk4", "pmsm_fin_sc_rk4", "scim_cc_rk4", "eesm_cc_rk4", "permex_cc_rk4"])
-def test_rollout_matches_oracle(torch_cuda, oracle_lib, name, dtype, tol):
-    """the rollout path against the CPU oracle directly (not only through the step kernel): full trajectory of 1000 envs x 60 steps"""
+ORACLE_NAMES = ["pmsm_cc_rk4", "pmsm_fin_sc_rk4", "scim_cc_rk4", "eesm_cc_rk4", "permex_cc_rk4"]
+# at the launch shapes of large batches (gpu_helpers.launch_sizes: 64- and 128-thread blocks) also a wrapper, a dead-time + RC + dq, an AC
+# supply, an external speed profile and a DFIM configuration
+ORACLE_CASES = [pytest.param(name, 1000, id=name) for name in ORACLE_NAMES] + [
+    pytest.param(name, size, id=f"{name}-{size}") for size in ("N64", "N128")
+    for name in ORACLE_NAMES + ["pmsm_cc_cossin_rk4", "eesm_cc_rc_dq_dead1_rk4", "pmsm_cc_ac_rk4", "pmsm_cc_extspeed_rk4", "dfim_cc_rk4"]]
+
+
+@pytest.mark.parametrize("dtype", [K.F64, K.F32], ids=["f64", "f32"])
+@pytest.mark.parametrize("name,n", ORACLE_CASES)
+def test_rollout_matches_oracle(torch_cuda, oracle_lib, name, n, dtype):
+    """the rollout path against the CPU oracle directly (not only through the step kernel): full trajectory of every env, 1000 envs x 60
+    steps, and whole batches of N64 / N128 envs (one-warp blocks no longer) x 12 steps"""
     torch = torch_cuda
     from gym_electric_motor_b200.vector_sim import VectorSim
 
-    n, k_total = 1000, 60
+    n, k_total = (n, 60) if n == 1000 else (launch_sizes()[n], 12)
+    tol = _tol(name, dtype)
     g, cfg = _mk(name, n, dtype, K.LAYOUT_AOS)
     _, cfg_o = _mk(name, n, K.F64, K.LAYOUT_AOS)
     sim, ora = VectorSim(cfg), oracle_lib.Oracle(cfg_o, nthreads=8)
@@ -107,17 +117,13 @@ def test_rollout_matches_oracle(torch_cuda, oracle_lib, name, dtype, tol):
     obs, ref, rew, term = [t.cpu().numpy() for t in sim.rollout(_dev_actions(torch, sim, acts), record_every=1)]
     alive = np.ones(n, dtype=bool)
     scale = np.full(obs.shape[2], 1e-3)
-    weak_dq = ((5, 6), (10, 11)) if name.startswith("scim") else ()
+    weak_dq = WEAK_DQ_PAIRS.get(cfg.motor_kind, ())
     for k in range(k_total):
         psi = ora.get_ode_state()[:, 3:5] if weak_dq else None
         o_obs, o_ref, o_rew, o_term = ora.step(acts[k])
         d_obs = obs[k].astype(np.float64)
         if weak_dq:  # field-frame columns while the rotor flux is ~0 (DESIGN.md finding 3): compare the magnitude
-            weak = np.hypot(psi[:, 0], psi[:, 1]) < 1e-3
-            for arr in (d_obs, o_obs):
-                for p_, q_ in weak_dq:
-                    arr[weak, p_] = np.hypot(arr[weak, p_], arr[weak, q_])
-                    arr[weak, q_] = 0.0
+            fold_weak_dq(weak_dq, np.hypot(psi[:, 0], psi[:, 1]) < 1e-3, d_obs, o_obs)
         alive &= ~(alive & (o_term != term[k]))  # a constraint within rounding of its threshold: the episodes diverge from here
         scale = np.maximum(scale, np.abs(o_obs[alive]).max(axis=0))
         diff = np.abs(d_obs - o_obs)
