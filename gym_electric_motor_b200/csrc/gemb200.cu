@@ -323,20 +323,22 @@ static int row_words(const Section& s) { return s.per_env * (s.esz == 8 ? 2 : 1)
 // ----------------------------------------------------------------------------------------------------------------
 // model constants (double) -> StepParams<real>
 // ----------------------------------------------------------------------------------------------------------------
+// A parameter row: one env's physical parameters in the slot order of praw, GEMB200_MAX_MOTOR_PARAM motor slots, then the 8 load slots.
+// NULL motor / load parameters: the configuration's.
+static void param_row(const gemb200_config& c, const double* motor_param, const double* load_param, double* row) {
+  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) row[s] = motor_param ? motor_param[s] : c.motor_param[s];
+  for (int s = 0; s < 8; ++s) row[GEMB200_MAX_MOTOR_PARAM + s] = load_param ? load_param[s] : c.load_param[s];
+}
+
 struct Derived {
-  double c[20] = {0};
-  double tq[4] = {0};
+  ModelCoef mc;
   double reset_obs[GEMB200_MAX_STATE] = {0};
   double reset_obs_du[GEMB200_MAX_STATE] = {0};  // d reset_obs / d u_sup (the voltage entries are linear in u_sup)
-  double inv_j = 0, omega_lim = 0, omega_lin = 0;
 };
 
 static void derive_model(const gemb200_config* cfg, const Dims& dm, Derived* o) {
-  ModelCoef mc;
-  derive_coef(cfg->motor_kind, cfg->motor_param, cfg->load_param, &mc);  // gemb200_model.h: shared with the parameter draws on the device
-  for (int j = 0; j < 20; ++j) o->c[j] = mc.c[j];
-  for (int j = 0; j < 4; ++j) o->tq[j] = mc.tq[j];
-  o->inv_j = mc.inv_j; o->omega_lim = mc.omega_lim; o->omega_lin = mc.omega_lin;
+  derive_coef(cfg->motor_kind, cfg->motor_param, cfg->load_param, &o->mc);  // gemb200_model.h: shared with the parameter draws on the device
+  const ModelCoef& mc = o->mc;
 
   // observation right after reset (SCMLSystem.reset physical_systems.py:256-287, :527-561, :659-693, :816-847) for the
   // constant initial state; converter.reset() gives 0 per QC and -0.5 per B6 leg (converters.py:45-54, :880-886)
@@ -346,9 +348,9 @@ static void derive_model(const gemb200_config* cfg, const Dims& dm, Derived* o) 
   int n = 0;
   s[n++] = y[0];
   switch (dm.fam) {
-    case kDC1: s[n++] = (o->tq[0] + o->tq[1] * y[1]) * y[1]; s[n++] = y[1]; s[n++] = 0.0; break;
+    case kDC1: s[n++] = (mc.tq[0] + mc.tq[1] * y[1]) * y[1]; s[n++] = y[1]; s[n++] = 0.0; break;
     case kDC2:
-      s[n++] = o->tq[0] * y[1] * y[2]; s[n++] = y[1]; s[n++] = y[2]; s[n++] = 0.0;
+      s[n++] = mc.tq[0] * y[1] * y[2]; s[n++] = y[1]; s[n++] = y[2]; s[n++] = 0.0;
       if (cfg->motor_kind == GEMB200_MOTOR_EXTEX_DC) s[n++] = 0.0;
       break;
     default: {
@@ -361,11 +363,11 @@ static void derive_model(const gemb200_config* cfg, const Dims& dm, Derived* o) 
       if (dm.fam == kSCIM || dm.fam == kDFIM) {
         const double ef = std::atan2(y[4], y[3]);
         cs = std::cos(ef); sn = std::sin(ef);
-        tqv = o->tq[0] * (y[3] * y[2] - y[4] * y[1]);
+        tqv = mc.tq[0] * (y[3] * y[2] - y[4] * y[1]);
         ia = y[1]; ib = y[2];
       } else {
         cs = std::cos(eps); sn = std::sin(eps);
-        tqv = dm.fam == kSYNC ? (o->tq[0] + o->tq[1] * y[1]) * y[2] : (o->tq[0] * y[3] + o->tq[1] * y[1]) * y[2];
+        tqv = dm.fam == kSYNC ? (mc.tq[0] + mc.tq[1] * y[1]) * y[2] : (mc.tq[0] * y[3] + mc.tq[1] * y[1]) * y[2];
         ia = cs * y[1] - sn * y[2]; ib = sn * y[1] + cs * y[2];
       }
       const double ud = cs * ualpha + sn * ubeta, uq = -sn * ualpha + cs * ubeta;
@@ -374,7 +376,7 @@ static void derive_model(const gemb200_config* cfg, const Dims& dm, Derived* o) 
       if (dm.fam == kDFIM) {
         // physical_systems.py:1062-1113: i_sdq in the field frame; i_rdq (sic) with the angle eps_field - eps_el, i_rdef = its inverse;
         // all six bridge legs at -0.5 u_sup, whose alpha-beta image is 0
-        const double ira = o->c[8] * y[3] - o->c[9] * y[1], irb = o->c[8] * y[4] - o->c[9] * y[2];
+        const double ira = mc.c[8] * y[3] - mc.c[9] * y[1], irb = mc.c[8] * y[4] - mc.c[9] * y[2];
         const double cfe = std::cos(std::atan2(y[4], y[3]) - eps), sfe = std::sin(std::atan2(y[4], y[3]) - eps);
         s[n++] = cs * y[1] + sn * y[2]; s[n++] = -sn * y[1] + cs * y[2];
         s[n++] = ira; s[n++] = -0.5 * ira + 0.5 * std::sqrt(3.0) * irb; s[n++] = -0.5 * ira - 0.5 * std::sqrt(3.0) * irb;
@@ -457,10 +459,7 @@ static bool fill_params(const gemb200_handle* h, const Dims& dm, const Derived& 
       }
     }
   }
-  for (int j = 0; j < 20; ++j) p->k.c[j] = (real)dv.c[j];
-  for (int j = 0; j < 4; ++j) p->k.tq[j] = (real)dv.tq[j];
-  p->k.load_a = (real)c.load_param[GEMB200_LP_A]; p->k.load_b = (real)c.load_param[GEMB200_LP_B]; p->k.load_c = (real)c.load_param[GEMB200_LP_C];
-  p->k.inv_j = (real)dv.inv_j; p->k.omega_lim = (real)dv.omega_lim; p->k.omega_lin = (real)dv.omega_lin;
+  coef_words(dv.mc, c.load_param, [p](int w, double v) { reinterpret_cast<real*>(&p->k)[w] = (real)v; });
   for (int j = 0; j < dm.n_state; ++j) {
     p->inv_lim[j] = c.limits[j] != 0.0 ? (real)(1.0 / c.limits[j]) : real(0);
     p->reset_obs[j] = (real)dv.reset_obs[j];
@@ -947,8 +946,7 @@ int gemb200_coef_tangents(const gemb200_config* cfg, const double* motor_param, 
   if (rc) return rc;
   if (const char* why = param_sens_refusal(cfg, n_p, slots)) return fail(GEMB200_E_INVALID, why);
   double prm[kMaxDraw];
-  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) prm[s] = motor_param ? motor_param[s] : cfg->motor_param[s];
-  for (int s = 0; s < 8; ++s) prm[GEMB200_MAX_MOTOR_PARAM + s] = load_param ? load_param[s] : cfg->load_param[s];
+  param_row(*cfg, motor_param, load_param, prm);
   for (int a = 0; a < n_p; ++a) coef_tangent(cfg->motor_kind, prm, slots[a], out + (size_t)a * kCoefWords);
   return GEMB200_OK;
 }
@@ -1139,8 +1137,7 @@ int gemb200_rollout_param_sens(gemb200_handle* h, const void* actions, const voi
   PsOut po{};
   po.sio = sens_io; po.sout = sens_out; po.np = n_p;
   for (int a = 0; a < n_p; ++a) po.slot[a] = slots[a];
-  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) po.raw[s] = h->cfg.motor_param[s];
-  for (int s = 0; s < 8; ++s) po.raw[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
+  param_row(h->cfg, nullptr, nullptr, po.raw);
   DeviceGuard guard(h->cfg.device);
   return do_step(h, actions, obs_out, ref_out, reward_out, terminated_out, (cudaStream_t)stream, 0, -1, true, n_steps, 1, references, nullptr, nullptr,
                  1.0, &po);
@@ -1151,111 +1148,20 @@ int gemb200_rollout(gemb200_handle* h, const void* actions, int32_t n_steps, voi
   return gemb200_rollout_record(h, actions, n_steps, 0, obs_out, ref_out, reward_out, terminated_out, stream);
 }
 
-// Domain randomisation (SURVEY.md §8f row 4; the batched counterpart of constructing N reference envs with N motor_parameter / load_parameter
-// dicts): every env gets its own model coefficients, derived here exactly like the shared ones (the *_update_model methods,
-// mechanical_load.py:188-193) from ITS physical parameters.  Limits, nominal values, reward and reference settings stay those of the
-// handle's configuration.  NULL motor_param: back to the shared coefficients.
-static int fill_shared_blocks(gemb200_handle* h);
-int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const double* load_param) {
-  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
-  DeviceGuard guard(h->cfg.device);
-  CUDA_TRY(cudaDeviceSynchronize());
-  if (h->cfg.layout != GEMB200_LAYOUT_AOS && (motor_param || load_param))
-    return fail(GEMB200_E_INVALID, "per-env parameter blocks need the row-per-env (AoS) I/O layout");
-  if (!motor_param && !load_param) {
-    h->n_draw = 0;  // shared coefficients again: no parameter draws either
-    int rc = GEMB200_OK;
-    if (h->ids_in_use) {  // adopted RNG identities are read by the ENVP instantiations only: the blocks take the shared parameters instead
-      rc = fill_shared_blocks(h);
-      if (!rc) h->blocks = kBlocksShared;
-    } else {
-      h->blocks = kBlocksNone;
-    }
-    apply_mode(h);
-    return rc;
-  }
-  const size_t n = (size_t)h->cfg.n_envs;
-  Dims d;
-  derive_dims(&h->cfg, &d);
-  std::vector<double> tab((size_t)kCoefWords * n);
-  std::vector<double> raw((size_t)kMaxDraw * n);  // the physical parameters themselves: what parameter draws at a reset start from
-  gemb200_config c = h->cfg;
-  for (size_t i = 0; i < n; ++i) {
-    if (motor_param) std::memcpy(c.motor_param, motor_param + i * GEMB200_MAX_MOTOR_PARAM, sizeof(c.motor_param));
-    if (load_param) std::memcpy(c.load_param, load_param + i * 8, sizeof(c.load_param));
-    if (c.motor_param[GEMB200_MP_P] != h->cfg.motor_param[GEMB200_MP_P])
-      return fail(GEMB200_E_INVALID, "pole pairs cannot differ per env: the angle increments are prepared on the host per handle");
-    for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw[(size_t)s * n + i] = c.motor_param[s];
-    for (int s = 0; s < 8; ++s) raw[(size_t)(GEMB200_MAX_MOTOR_PARAM + s) * n + i] = c.load_param[s];
-    if (c.load_kind == GEMB200_LOAD_POLY_STATIC && !(c.load_param[GEMB200_LP_J_LOAD] + c.motor_param[GEMB200_MP_J_ROTOR] > 0))
-      return fail(GEMB200_E_INVALID, "per-env parameters: total inertia must be positive for every env");
-    Derived dv;
-    derive_model(&c, d, &dv);
-    for (int w = 0; w < 20; ++w) tab[(size_t)w * n + i] = dv.c[w];
-    for (int w = 0; w < 4; ++w) tab[(size_t)(20 + w) * n + i] = dv.tq[w];
-    tab[(size_t)24 * n + i] = c.load_param[GEMB200_LP_A]; tab[(size_t)25 * n + i] = c.load_param[GEMB200_LP_B]; tab[(size_t)26 * n + i] = c.load_param[GEMB200_LP_C];
-    tab[(size_t)27 * n + i] = dv.inv_j; tab[(size_t)28 * n + i] = dv.omega_lim; tab[(size_t)29 * n + i] = dv.omega_lin;
-  }
-  for (double v : tab) if (!std::isfinite(v)) return fail(GEMB200_E_INVALID, "per-env parameters: a derived model coefficient is not finite (zero inductance?)");
-  if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, tab.size() * h->rsz));
-  if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, raw.size() * sizeof(double)));
-  CUDA_TRY(cudaMemcpy(h->d_praw, raw.data(), raw.size() * sizeof(double), cudaMemcpyHostToDevice));
-  const int rc = with_params(h, [&](auto& p) {
-    using real = decltype(p.tau);
-    const std::vector<real> t(tab.begin(), tab.end());
-    CUDA_TRY(cudaMemcpy(h->d_envp, t.data(), t.size() * sizeof(real), cudaMemcpyHostToDevice));
-    return GEMB200_OK;
-  });
-  if (rc) return rc;
-  h->blocks = kBlocksCaller;
-  apply_mode(h);
-  return GEMB200_OK;
-}
-
 }  // extern "C"
 
 // Per-env parameter blocks filled on the device from the shared configuration: every env gets the shared coefficients (the values
-// gemb200_set_env_params derives from rows equal to the configuration's) and the configuration's physical parameters.
+// gemb200_set_env_params derives from rows equal to the configuration's), copied word by word (Coef is the block's word order), and the
+// configuration's physical parameters.
 struct RawParams { double v[kMaxDraw]; };
 template <typename real>
 __global__ void fill_env_params_kernel(real* envp, double* praw, const Coef<real> k, const RawParams raw, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const size_t nn = (size_t)n;
-  for (int w = 0; w < 20; ++w) envp[w * nn + i] = k.c[w];
-  for (int w = 0; w < 4; ++w) envp[(20 + w) * nn + i] = k.tq[w];
-  envp[24 * nn + i] = k.load_a; envp[25 * nn + i] = k.load_b; envp[26 * nn + i] = k.load_c;
-  envp[27 * nn + i] = k.inv_j; envp[28 * nn + i] = k.omega_lim; envp[29 * nn + i] = k.omega_lin;
+  const real* kw = reinterpret_cast<const real*>(&k);
+  for (int w = 0; w < kCoefWords; ++w) envp[w * nn + i] = kw[w];
   for (int s = 0; s < kMaxDraw; ++s) praw[s * nn + i] = raw.v[s];
-}
-// the configuration's physical parameters in the slot order of praw
-static RawParams config_params(const gemb200_handle* h) {
-  RawParams raw;
-  for (int s = 0; s < GEMB200_MAX_MOTOR_PARAM; ++s) raw.v[s] = h->cfg.motor_param[s];
-  for (int s = 0; s < 8; ++s) raw.v[GEMB200_MAX_MOTOR_PARAM + s] = h->cfg.load_param[s];
-  return raw;
-}
-// no adopted identities any more: launches key every env by its own identity again, and blocks that only an adoption made go, so that the
-// handle runs its shared-coefficient kernels like a fresh one (the identity array stays allocated for the next adoption)
-static void drop_rng_ids(gemb200_handle* h) {
-  h->ids_in_use = false;
-  if (h->blocks == kBlocksShared) h->blocks = kBlocksNone;
-  apply_mode(h);
-}
-// every env's block := the shared parameters (synchronises); the caller sets the handle's blocks and applies the mode
-static int fill_shared_blocks(gemb200_handle* h) {
-  const size_t nn = (size_t)h->cfg.n_envs;
-  if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
-  if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, (size_t)kMaxDraw * nn * sizeof(double)));
-  const RawParams raw = config_params(h);
-  const int grid = (int)((nn + 255) / 256);
-  with_params(h, [&](auto& p) {
-    using real = decltype(p.tau);
-    fill_env_params_kernel<real><<<grid, 256>>>(static_cast<real*>(h->d_envp), h->d_praw, p.k, raw, (int)nn);
-  });
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaDeviceSynchronize());
-  return GEMB200_OK;
 }
 // out[j][i] = stored value of drawn parameter j of env i, in the handle's dtype
 template <typename real>
@@ -1264,8 +1170,80 @@ __global__ void get_env_params_kernel(const double* praw, const ParamDraw* d, in
   if (i >= n) return;
   for (int j = 0; j < n_draw; ++j) out[(size_t)j * n + i] = (real)praw[(size_t)d->slot[j] * n + i];
 }
+static RawParams config_params(const gemb200_handle* h) {
+  RawParams raw;
+  param_row(h->cfg, nullptr, nullptr, raw.v);
+  return raw;
+}
+// The per-env parameter blocks d_envp / d_praw of a handle come from `to` afterwards; every change of them goes through here.  Blocks are
+// allocated at their first use.  Blocks that are new, or the caller's that become Shared, get the configuration's parameters (synchronises),
+// unless the caller writes every env's block right after (`overwritten`); Shared blocks hold them already.  Then the launch mode follows.
+static int use_blocks(gemb200_handle* h, BlockSource to, bool overwritten = false) {
+  const size_t nn = (size_t)h->cfg.n_envs;
+  if (to != kBlocksNone) {
+    if (!h->d_envp) CUDA_TRY(cudaMalloc(&h->d_envp, (size_t)kCoefWords * nn * h->rsz));
+    if (!h->d_praw) CUDA_TRY(cudaMalloc(&h->d_praw, (size_t)kMaxDraw * nn * sizeof(double)));
+    if (to != h->blocks && h->blocks != kBlocksShared && !overwritten) {
+      const RawParams raw = config_params(h);
+      const int grid = (int)((nn + 255) / 256);
+      with_params(h, [&](auto& p) {
+        using real = decltype(p.tau);
+        fill_env_params_kernel<real><<<grid, 256>>>(static_cast<real*>(h->d_envp), h->d_praw, p.k, raw, (int)nn);
+      });
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(cudaDeviceSynchronize());
+    }
+  }
+  h->blocks = to;
+  apply_mode(h);
+  return GEMB200_OK;
+}
 
 extern "C" {
+
+// Domain randomisation (SURVEY.md §8f row 4; the batched counterpart of constructing N reference envs with N motor_parameter / load_parameter
+// dicts): every env gets its own model coefficients, derived here exactly like the shared ones (the *_update_model methods,
+// mechanical_load.py:188-193) from ITS physical parameters.  Limits, nominal values, reward and reference settings stay those of the
+// handle's configuration.  NULL motor_param: back to the shared coefficients.
+int gemb200_set_env_params(gemb200_handle* h, const double* motor_param, const double* load_param) {
+  if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
+  DeviceGuard guard(h->cfg.device);
+  CUDA_TRY(cudaDeviceSynchronize());
+  if (h->cfg.layout != GEMB200_LAYOUT_AOS && (motor_param || load_param))
+    return fail(GEMB200_E_INVALID, "per-env parameter blocks need the row-per-env (AoS) I/O layout");
+  if (!motor_param && !load_param) {
+    h->n_draw = 0;  // shared coefficients again: no parameter draws either
+    // adopted RNG identities are read by the ENVP instantiations only: the blocks take the shared parameters instead
+    return use_blocks(h, h->ids_in_use ? kBlocksShared : kBlocksNone);
+  }
+  const gemb200_config& c = h->cfg;
+  const size_t n = (size_t)c.n_envs;
+  std::vector<double> tab((size_t)kCoefWords * n);
+  std::vector<double> raw((size_t)kMaxDraw * n);  // the physical parameters themselves: what parameter draws at a reset start from
+  for (size_t i = 0; i < n; ++i) {
+    double row[kMaxDraw];
+    param_row(c, motor_param ? motor_param + i * GEMB200_MAX_MOTOR_PARAM : nullptr, load_param ? load_param + i * 8 : nullptr, row);
+    const double *mp = row, *lp = row + GEMB200_MAX_MOTOR_PARAM;
+    if (mp[GEMB200_MP_P] != c.motor_param[GEMB200_MP_P])
+      return fail(GEMB200_E_INVALID, "pole pairs cannot differ per env: the angle increments are prepared on the host per handle");
+    for (int s = 0; s < kMaxDraw; ++s) raw[(size_t)s * n + i] = row[s];
+    if (c.load_kind == GEMB200_LOAD_POLY_STATIC && !(lp[GEMB200_LP_J_LOAD] + mp[GEMB200_MP_J_ROTOR] > 0))
+      return fail(GEMB200_E_INVALID, "per-env parameters: total inertia must be positive for every env");
+    ModelCoef mc;
+    derive_coef(c.motor_kind, mp, lp, &mc);
+    coef_words(mc, lp, [&](int w, double v) { tab[(size_t)w * n + i] = v; });
+  }
+  for (double v : tab) if (!std::isfinite(v)) return fail(GEMB200_E_INVALID, "per-env parameters: a derived model coefficient is not finite (zero inductance?)");
+  const int rc = use_blocks(h, kBlocksCaller, true);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpy(h->d_praw, raw.data(), raw.size() * sizeof(double), cudaMemcpyHostToDevice));
+  return with_params(h, [&](auto& p) {
+    using real = decltype(p.tau);
+    const std::vector<real> t(tab.begin(), tab.end());
+    CUDA_TRY(cudaMemcpy(h->d_envp, t.data(), t.size() * sizeof(real), cudaMemcpyHostToDevice));
+    return GEMB200_OK;
+  });
+}
 
 int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t* slot, const int32_t* kind, const double* lo, const double* hi) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
@@ -1301,11 +1279,8 @@ int gemb200_set_param_randomization(gemb200_handle* h, int32_t n, const int32_t*
   }
   if (!h->d_draw) CUDA_TRY(cudaMalloc(&h->d_draw, sizeof(ParamDraw)));
   CUDA_TRY(cudaMemcpy(h->d_draw, &pd, sizeof(pd), cudaMemcpyHostToDevice));
-  if (h->blocks == kBlocksNone) {  // no per-env blocks yet: every env starts from the shared parameters
-    const int rc = fill_shared_blocks(h);
-    if (rc) return rc;
-  }
-  h->blocks = kBlocksCaller;  // the draws change the blocks: they are the caller's from now on
+  const int rc = use_blocks(h, kBlocksCaller);  // the draws change the blocks: they are the caller's from now on
+  if (rc) return rc;
   h->n_draw = n;
   apply_mode(h);
   return GEMB200_OK;
@@ -1605,7 +1580,8 @@ int gemb200_reseed(gemb200_handle* h, uint64_t seed, void* stream) {
   h->gstep = 0; h->n_steps = 0;
   if (h->dev_clock) { int rc = push_clock(h, st); if (rc) return rc; }
   with_params(h, [&](auto& p) { set_seed(&p, seed); });
-  drop_rng_ids(h);  // every env draws with its own identity again
+  h->ids_in_use = false;  // every env draws with its own identity again (see gemb200_clear_rng_ids)
+  use_blocks(h, h->blocks == kBlocksShared ? kBlocksNone : h->blocks);
   Section s[kMaxSections];
   const int k = sections(h, s);
   for (int i = 0; i < k; ++i) {
@@ -2032,9 +2008,8 @@ static int adopt_rng_id_rows(gemb200_handle* h, const uint32_t* ids, int32_t n_i
   if (!ids) return fail(GEMB200_E_INVALID, "ids is NULL");
   DeviceGuard guard(h->cfg.device);
   if (h->blocks == kBlocksNone) {  // first adoption: the shared parameters into per-env blocks, so that the handle runs the ENVP instantiations (synchronises)
-    const int rc = fill_shared_blocks(h);
+    const int rc = use_blocks(h, kBlocksShared);
     if (rc) return rc;
-    h->blocks = kBlocksShared;
   }
   if (!h->d_rngid) CUDA_TRY(cudaMalloc(&h->d_rngid, (size_t)kRngIdWords * (size_t)h->cfg.n_envs * sizeof(uint32_t)));
   if (!h->ids_in_use) {  // every other env keeps its own identity
@@ -2076,8 +2051,10 @@ int gemb200_adopt_rng_ids(gemb200_handle* h, const uint32_t* ids, int32_t n_ids,
 int gemb200_clear_rng_ids(gemb200_handle* h, void* stream) {
   if (!h) return fail(GEMB200_E_INVALID, "handle is NULL");
   (void)stream;  // launches enqueued before the call keep the identities they were launched with
-  drop_rng_ids(h);
-  return GEMB200_OK;
+  // launches key every env by its own identity again, and blocks that only an adoption made go, so that the handle runs its
+  // shared-coefficient kernels like a fresh one (the identity array stays allocated for the next adoption)
+  h->ids_in_use = false;
+  return use_blocks(h, h->blocks == kBlocksShared ? kBlocksNone : h->blocks);
 }
 
 }  // extern "C"
@@ -2121,25 +2098,8 @@ __global__ void __launch_bounds__(kParBlock) pack_env_params_kernel(const double
   }
 }
 
-// Env i's column of the per-env parameter block envp [kCoefWords][n], derived from its physical parameters prm[kMaxDraw] by derive_coef
-// (gemb200_model.h), the derivation of the parameter draws and of gemb200_set_env_params.  The same stores end redraw_env_params
-// (gemb200_kernels.cuh); calling this function from there changes the register allocation of every reset kernel and ENVP step / rollout
-// kernel of the step translation units (DESIGN §4), so the eight lines are kept in both places.
-template <typename real>
-__device__ __forceinline__ void write_env_coef(int motor_kind, const double* prm, real* envp, unsigned i, size_t n) {
-  ModelCoef mc;
-  derive_coef(motor_kind, prm, prm + GEMB200_MAX_MOTOR_PARAM, &mc);
-  real* e = envp + i;
-  for (int w = 0; w < 20; ++w) e[(size_t)w * n] = (real)mc.c[w];
-  for (int w = 0; w < 4; ++w) e[(size_t)(20 + w) * n] = (real)mc.tq[w];
-  e[(size_t)24 * n] = (real)prm[GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_A];
-  e[(size_t)25 * n] = (real)prm[GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_B];
-  e[(size_t)26 * n] = (real)prm[GEMB200_MAX_MOTOR_PARAM + GEMB200_LP_C];
-  e[(size_t)27 * n] = (real)mc.inv_j; e[(size_t)28 * n] = (real)mc.omega_lim; e[(size_t)29 * n] = (real)mc.omega_lin;
-}
-
 // env env_idx[j] (NULL: j) takes parameter row row_idx[j] (NULL: j): every slot but the pole pairs (per handle: the angle increments are
-// prepared on the host) into praw, and the coefficients derived from them into its envp column (write_env_coef, as a parameter draw does)
+// prepared on the host) into praw, and the coefficients derived from them (derive_coef, as a parameter draw does) into its envp column
 template <typename real>
 __global__ void __launch_bounds__(kParBlock) adopt_env_params_kernel(double* __restrict__ praw, real* __restrict__ envp, int n, int motor_kind,
                                                                      const double* __restrict__ rows, int n_rows, const int32_t* __restrict__ row_idx,
@@ -2172,7 +2132,10 @@ __global__ void __launch_bounds__(kParBlock) adopt_env_params_kernel(double* __r
 #pragma unroll
   for (int s = 0; s < kMaxDraw; ++s)
     if (s != GEMB200_MP_P) praw[(size_t)s * nn + i] = prm[s];
-  write_env_coef<real>(motor_kind, prm, envp, (unsigned)i, nn);
+  ModelCoef mc;
+  derive_coef(motor_kind, prm, prm + GEMB200_MAX_MOTOR_PARAM, &mc);
+  real* e = envp + (unsigned)i;
+  coef_words(mc, prm + GEMB200_MAX_MOTOR_PARAM, [&](int w, double v) { e[(size_t)w * nn] = (real)v; });
 }
 
 extern "C" {
@@ -2201,12 +2164,8 @@ int gemb200_unpack_envs_params(gemb200_handle* h, const uint32_t* rows, const do
   if (rc || m == 0 || n_rows == 0) return rc;
   DeviceGuard guard(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (h->blocks == kBlocksNone) {  // no per-env blocks yet: every other env keeps the shared parameters (synchronises)
-    rc = fill_shared_blocks(h);
-    if (rc) return rc;
-  }
-  h->blocks = kBlocksCaller;  // the blocks hold rows of the caller's now
-  apply_mode(h);
+  rc = use_blocks(h, kBlocksCaller);  // the blocks hold rows of the caller's now; every other env keeps its parameters
+  if (rc) return rc;
   rc = unpack_env_rows(h, rows, n_rows, layout_id, row_idx, env_idx, m, stream);
   if (rc) return rc;
   with_params(h, [&](auto& p) {

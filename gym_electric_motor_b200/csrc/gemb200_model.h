@@ -5,6 +5,7 @@
 // without FMA contraction, so both sides round every operation the same way and the device result equals the host result bit for bit.
 #pragma once
 #include "../../include/gemb200.h"
+#include "gemb200_params.h"
 
 namespace gemb200 {
 
@@ -96,9 +97,21 @@ __host__ __device__ inline void derive_coef_t(int motor_kind, const T* mp, const
 
 __host__ __device__ inline void derive_coef(int motor_kind, const double* mp, const double* lp, ModelCoef* o) { derive_coef_t<double>(motor_kind, mp, lp, o); }
 
-// d (coefficient block) / d prm[slot] in the word order of Coef (kCoefWords = 30: c[20], tq[4], load_a, load_b, load_c, inv_j, omega_lim,
-// omega_lin), prm = the env's physical parameters in the slot order of a parameter row (GEMB200_MAX_MOTOR_PARAM motor slots, then 8 load
-// slots).  The load words a, b, c are the parameters themselves.  Not inlined on the device: it runs once per launch and env, and its
+// The column of one env's coefficient block, in the word order of Coef (gemb200_params.h): put(w, value) for each of the kCoefWords words,
+// from the derived coefficients o and the env's load slots lp (the load polynomial's a, b, c are block words themselves).  Every block
+// column and the shared coefficients are written through it, except in redraw_env_params (gemb200_kernels.cuh), which spells its stores
+// out (DESIGN §4).  `put` runs where the caller runs (host or device): no execution-space check on it.
+#pragma nv_exec_check_disable
+template <typename T, typename Put>
+__host__ __device__ inline void coef_words(const ModelCoefT<T>& o, const T* lp, Put&& put) {
+  for (int w = 0; w < kCwTq; ++w) put(w, o.c[w]);
+  for (int w = 0; w < kCwLoad - kCwTq; ++w) put(kCwTq + w, o.tq[w]);
+  put(kCwLoad, lp[GEMB200_LP_A]); put(kCwLoad + 1, lp[GEMB200_LP_B]); put(kCwLoad + 2, lp[GEMB200_LP_C]);
+  put(kCwLoad + 3, o.inv_j); put(kCwLoad + 4, o.omega_lim); put(kCwLoad + 5, o.omega_lin);
+}
+
+// d (coefficient block) / d prm[slot] in the word order of Coef, prm = the env's physical parameters in the slot order of a parameter row
+// (GEMB200_MAX_MOTOR_PARAM motor slots, then 8 load slots).  Not inlined on the device: it runs once per launch and env, and its
 // double-precision body stays out of the kernels' step loop.
 __host__ __device__ __noinline__ inline void coef_tangent(int motor_kind, const double* prm, int slot, double* out) {
   Dual m[GEMB200_MAX_MOTOR_PARAM], l[8];
@@ -106,10 +119,7 @@ __host__ __device__ __noinline__ inline void coef_tangent(int motor_kind, const 
   for (int s = 0; s < 8; ++s) l[s] = Dual(prm[GEMB200_MAX_MOTOR_PARAM + s], GEMB200_MAX_MOTOR_PARAM + s == slot ? 1.0 : 0.0);
   ModelCoefT<Dual> o;
   derive_coef_t<Dual>(motor_kind, m, l, &o);
-  for (int w = 0; w < 20; ++w) out[w] = o.c[w].d;
-  for (int w = 0; w < 4; ++w) out[20 + w] = o.tq[w].d;
-  out[24] = l[GEMB200_LP_A].d; out[25] = l[GEMB200_LP_B].d; out[26] = l[GEMB200_LP_C].d;
-  out[27] = o.inv_j.d; out[28] = o.omega_lim.d; out[29] = o.omega_lin.d;
+  coef_words(o, l, [out](int w, Dual v) { out[w] = v.d; });
 }
 
 }  // namespace gemb200

@@ -81,16 +81,27 @@ constexpr bool streams_disjoint() {
 }
 static_assert(streams_disjoint(), "RNG stream id ranges overlap");
 
-// Model coefficients of ONE env: the motor's sparse constant matrix (layout per family, gemb200.cu: derive_model), torque coefficients,
+// Model coefficients of ONE env: the motor's sparse constant matrix (layout per family, gemb200_model.h: derive_coef), torque coefficients,
 // load polynomial and inertia.  Shared by the whole batch in the constant bank (StepParams::k) — or, with per-env parameter blocks
 // (gemb200_set_env_params: domain randomisation), loaded per thread from StepParams::envp.
-constexpr int kCoefWords = 30;
+// The same 30 words are a per-env block's column: word w of Coef is word w of the block (c at 0, tq at kCwTq, then the six load words a, b, c,
+// inv_j, omega_lim, omega_lin at kCwLoad ..  kCwLoad + 5).
+constexpr int kCoefWords = 30, kCwTq = 20, kCwLoad = 24;
 template <typename real>
 struct Coef {
   real c[20];  // motor model coefficients
   real tq[4];  // torque coefficients
   real load_a, load_b, load_c, inv_j, omega_lim, omega_lin;
 };
+template <typename real>
+constexpr bool coef_layout() {
+  return offsetof(Coef<real>, tq) == kCwTq * sizeof(real) && offsetof(Coef<real>, load_a) == kCwLoad * sizeof(real) &&
+         offsetof(Coef<real>, omega_lin) == (kCwLoad + 5) * sizeof(real) && sizeof(Coef<real>) == kCoefWords * sizeof(real);
+}
+static_assert(coef_layout<float>() && coef_layout<double>(), "Coef is the word order of a per-env block");
+// the words of c and of tq that family fam reads (derive_coef leaves the others 0)
+__host__ __device__ constexpr int coef_nc(int fam) { return fam == kDC1 ? 4 : (fam == kDC2 ? 5 : (fam == kSYNC ? 7 : (fam == kEESM ? 14 : 10))); }
+__host__ __device__ constexpr int coef_ntq(int fam) { return (fam == kDC2 || fam == kSCIM || fam == kDFIM) ? 1 : 2; }
 
 // Distributions of the parameters drawn at every reset (gemb200_set_param_randomization), in device memory behind StepParams::draw.
 // Draw j: v = a + b * U (uniform: a = lo, b = hi - lo; log-uniform: exp of it, a = log lo, b = log hi - log lo), clamped to [lo, hi].

@@ -436,17 +436,17 @@ __device__ __forceinline__ real reward_t(const StepParams<real>& p, const Coef<r
 
 // Parameter sensitivities: the words of the coefficient block (Coef, kCoefWords) that family FAM reads — load_coef's c and tq words and the
 // six load / inertia words — kept per parameter column in the staging row; word w of that compact list is word ps_word<FAM>(w) of Coef
-template <int FAM> __host__ __device__ constexpr int ps_ncw() { return FAM == kDC1 ? 4 : (FAM == kDC2 ? 5 : (FAM == kSYNC ? 7 : (FAM == kEESM ? 14 : 10))); }
-template <int FAM> __host__ __device__ constexpr int ps_ntq() { return (FAM == kDC2 || FAM == kSCIM || FAM == kDFIM) ? 1 : 2; }
-template <int FAM> __host__ __device__ constexpr int ps_words() { return ps_ncw<FAM>() + ps_ntq<FAM>() + 6; }
-template <int FAM> __host__ __device__ constexpr int ps_word(int w) { return w < ps_ncw<FAM>() ? w : (w < ps_ncw<FAM>() + ps_ntq<FAM>() ? 20 + w - ps_ncw<FAM>() : 24 + w - ps_ncw<FAM>() - ps_ntq<FAM>()); }
+template <int FAM> __host__ __device__ constexpr int ps_words() { return coef_nc(FAM) + coef_ntq(FAM) + kCoefWords - kCwLoad; }
+template <int FAM> __host__ __device__ constexpr int ps_word(int w) {
+  return w < coef_nc(FAM) ? w : (w < coef_nc(FAM) + coef_ntq(FAM) ? kCwTq + w - coef_nc(FAM) : kCwLoad + w - coef_nc(FAM) - coef_ntq(FAM));
+}
 template <int FAM, typename real>
 __device__ __forceinline__ void ps_coef(const real* t, Coef<real>& tk) {
 #pragma unroll
-  for (int w = 0; w < ps_ncw<FAM>(); ++w) tk.c[w] = t[w];
+  for (int w = 0; w < coef_nc(FAM); ++w) tk.c[w] = t[w];
 #pragma unroll
-  for (int w = 0; w < ps_ntq<FAM>(); ++w) tk.tq[w] = t[ps_ncw<FAM>() + w];
-  const real* m = t + ps_ncw<FAM>() + ps_ntq<FAM>();
+  for (int w = 0; w < coef_ntq(FAM); ++w) tk.tq[w] = t[coef_nc(FAM) + w];
+  const real* m = t + coef_nc(FAM) + coef_ntq(FAM);
   tk.load_a = m[0]; tk.load_b = m[1]; tk.load_c = m[2]; tk.inv_j = m[3]; tk.omega_lim = m[4]; tk.omega_lin = m[5];
 }
 
